@@ -60,7 +60,7 @@ def read_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler:
@@ -208,8 +208,8 @@ class Token:
         # launch list.  k+v and gate+up share their input and shape: the reference's model code issues them as ONE
         # exl3_mgemm each at bsz*q_len <= 32 (modules/attn.py:603-631 multi_kv, modules/mlp.py:726-760 multi_gu) whenever
         # config.use_mgemm() says so (model/config.py:48-64): always for narrow outputs (k+v), and for gate+up when
-        # ext.exl3_gemv_int8_max_k(device) < K -- the reference's own extension answers 6 on Blackwell (its separate int8 GEMVs
-        # beat its fused kernel), this library's shim answers 0 (the fused launch is the faster one here), so through the
+        # ext.exl3_gemv_int8_max_k(device) < K -- the reference's own extension answers 6 on Hopper (its separate int8 GEMVs
+        # beat its fused kernel), this library's shim answers 0 (one launch of the same kernel here), so through the
         # drop-in boundary the model issues exactly this launch list.  --no-fuse times one launch per projection.
         #
         # Fan-out (default; --no-fanout = the list above): q, k and v read the same input too, but q is wider than k / v.  The
@@ -226,6 +226,20 @@ class Token:
         if mode != "ops":
             self.build_chains(mode)
 
+    def outputs(self):
+        """Every output a caller of the timed token receives, by matrix ("L07_gate", ..., "lm_head"): the matrix's own y, or its
+        row of a multi-matrix call's output buffer."""
+        key = lambda mt: "lm_head" if mt["layer"] < 0 else f"L{mt['layer']:02d}_{mt['name']}"
+        out = {}
+        if self.mode != "ops":                              # chains write every matrix's own y
+            for mt in self.mats:
+                out[key(mt)] = mt["y"]
+            return out
+        for ln in self.launches:
+            for j, mt in enumerate(ln["mats"]):
+                out[key(mt)] = ln["y"][j].view(1, -1) if ln["kind"] == "mgemm" and ln["cp"] is None else mt["y"]
+        return out
+
     def _launch_list(self, fuse, fanout):
         torch, dev = self.torch, self.dev
         out = []
@@ -241,17 +255,18 @@ class Token:
                 out.append(dict(kind="mgemm", x=a["x"].view(1, 1, -1), K=a["K"], reduce=False, B=ptr("tr"), suh=ptr("suh"), svh=ptr("svh"),
                                 y=torch.empty((3, 1, max(t["n"] for t in grp)), dtype=a["y"].dtype, device=dev),     # dtype / max-width carrier
                                 xh=torch.empty((3, 1, a["k"]), dtype=torch.half, device=dev),
-                                snl=torch.tensor([t["n"] for t in grp], dtype=torch.int, device=dev), cp=ptr("y"), shared_inputs=3))
+                                snl=torch.tensor([t["n"] for t in grp], dtype=torch.int, device=dev), cp=ptr("y"), shared_inputs=3,
+                                mats=grp))
                 i += 3
             elif fuse and b is not None and (a["name"], b["name"]) in (("k", "v"), ("gate", "up")) and a["layer"] == b["layer"]:
                 ptr = lambda key: torch.tensor([a[key].data_ptr(), b[key].data_ptr()], dtype=torch.long, device=dev)
                 y2 = torch.empty((2, 1, a["n"]), dtype=a["y"].dtype, device=dev)
                 xh2 = torch.empty((2, 1, a["k"]), dtype=torch.half, device=dev)
                 out.append(dict(kind="mgemm", x=a["x"].view(1, 1, -1), y=y2, xh=xh2, K=a["K"], reduce=False,
-                                B=ptr("tr"), suh=ptr("suh"), svh=ptr("svh"), snl=None, cp=None, shared_inputs=2))
+                                B=ptr("tr"), suh=ptr("suh"), svh=ptr("svh"), snl=None, cp=None, shared_inputs=2, mats=(a, b)))
                 i += 2
             else:
-                out.append(dict(kind="gemm", mt=a, reduce=a["reduce"]))
+                out.append(dict(kind="gemm", mt=a, reduce=a["reduce"], mats=(a,)))
                 i += 1
         return out
 
@@ -339,7 +354,7 @@ def qgemm_section(tok, cfg, stream, hbm_peak):
       decode_hbm      per matrix shape of the model, the batch-1 qgemm's achieved HBM GB/s = algorithmic bytes (SURVEY.md 8d) /
                       launch time, from one CUDA-graph replay of that shape's 32 layer instances back to back (distinct weight
                       buffers, 67-940 MB per shape; weights are loaded evict-first), CUDA events on the launching stream
-      prefill_tensor  the prefill sibling of the same linear (reconstruct_had + tcgen05 dense GEMM, QLinear.forward for
+      prefill_tensor  the prefill sibling of the same linear (reconstruct_had + wgmma dense GEMM, QLinear.forward for
                       rows > 144) at batch 32 x 2048 rows: achieved TFLOP/s (2 m k n) against the measured dense bf16 peaks
     """
     import torch
@@ -376,7 +391,7 @@ def qgemm_section(tok, cfg, stream, hbm_peak):
                                    "GBps": round(b / best / 1e3, 1), "frac_of_hbm_peak": round(b / best / 1e3 / hbm_peak, 3),
                                    "distinct_weight_MB": round(len(mats) * mt["k"] * mt["n"] * mt["K"] / 8 / 1e6)}
         del g
-    # batch 8 / 32 decode (BASELINE config 3) on the default path: exact tcgen05 kernel, one launch per call
+    # batch 8 / 32 decode (BASELINE config 3) on the default path: exact tensor-core kernel, one launch per call
     out["decode_batch"] = {}
     for name in ("q", "gate", "down"):
         mats = by_name[name]
@@ -406,7 +421,7 @@ def qgemm_section(tok, cfg, stream, hbm_peak):
             out["decode_batch"][f"{name}_m{m}"] = {"us_per_launch": round(best, 2), "GBps": round(b / best / 1e3, 1),
                                                     "frac_of_hbm_peak": round(b / best / 1e3 / hbm_peak, 3), "tag": int(tag[0])}
             del g
-    # the other two codebooks at batch 1 (default path: exact tcgen05 kernel): same bytes, different decode
+    # the other two codebooks at batch 1 (default path: exact tensor-core kernel): same bytes, different decode
     out["decode_codebooks"] = {}
     for name in ("q", "gate"):
         mats = by_name[name]
@@ -436,7 +451,7 @@ def qgemm_section(tok, cfg, stream, hbm_peak):
             out["decode_codebooks"][f"{name}_{cbn}"] = {"us_per_launch": round(best, 2), "GBps": round(b / best / 1e3, 1),
                                                         "frac_of_hbm_peak": round(b / best / 1e3 / hbm_peak, 3), "tag": int(tag[0])}
             del g
-    # the reference's own CUDA kernels (unmodified sources compiled for sm_100a, oracle/_ref) on this GPU in this run, its default
+    # the reference's own CUDA kernels (unmodified sources compiled for sm_90a, oracle/_ref) on this GPU in this run, its default
     # configuration, same shapes and method (graph replay over >= 512 MB of rotated weight copies): the bar the kernels are held to
     ref_so = os.path.join(ROOT, "oracle", "_ref", "exl3_ref_ext.so")
     if os.path.exists(ref_so) and not os.environ.get("EXL3B_BENCH_NO_REF_CUDA"):
@@ -481,7 +496,7 @@ def qgemm_section(tok, cfg, stream, hbm_peak):
         d = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         peaks = {"burst": float(d["bf16_tflops"]), "sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"]))}
     except Exception:
-        peaks = {"burst": 2250.0, "sustained": 2250.0}          # nominal dense bf16 (B200_PROFILING.md fallback)
+        peaks = {"burst": 989.0, "sustained": 989.0}            # H100 SXM data sheet, dense bf16 (not measured)
     dev = tok.dev
     gen = torch.Generator(device=dev); gen.manual_seed(7)
     h = cfg["hidden"]
@@ -506,33 +521,17 @@ def qgemm_section(tok, cfg, stream, hbm_peak):
         out["prefill_tensor"][f"{k}x{n}_m{m}"] = {"rows": m, "ms": round(ms, 3), "tflops": round(tf, 1),
                                                    "frac_of_measured_bf16_burst": round(tf / peaks["burst"], 3),
                                                    "frac_of_measured_bf16_sustained": round(tf / peaks["sustained"], 3),
-                                                   "path": "reconstruct_had + tcgen05 dense GEMM (includes the weight reconstruction every call)"}
+                                                   "path": "reconstruct_had + wgmma dense GEMM (includes the weight reconstruction every call)"}
         del x, y, lin
     return out
 
 
-NCU_CAPTURE = os.path.join("profiles", "r02_ncu_gate.csv")     # metric,unit,value rows of one --set full capture
-
-
-def ncu_dram_bytes(path):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the committed ncu capture, in bytes (units as ncu printed them)."""
-    import csv
-    mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    cap = {r[0]: (r[1], r[2]) for r in csv.reader(open(path)) if len(r) == 3}
-    total = 0.0
-    for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-        unit, val = cap[key]
-        total += float(val) * mult[unit]
-    return total
-
-
-def ncu_traffic_per_launch(tok):
-    """DRAM traffic of the dominant kernel from the committed ncu capture (profiles/): measured bytes / algorithmic bytes of
-    the captured launch (gate shape), applied to the average launch of this step; None if the capture is missing."""
-    try:
-        return ncu_dram_bytes(os.path.join(ROOT, NCU_CAPTURE)) / alg_bytes(1, 4096, 14336, 4, True) * tok.alg_bytes / len(tok.launches)
-    except Exception:
-        return None
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: each array as out_dir/<name>.npy in float32 (the arrays a caller of the timed path receives)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy().astype(np.float32))
 
 
 def run_gpu_arm(args, cfg):
@@ -626,6 +625,10 @@ def run_gpu_arm(args, cfg):
     ms = timed(step, args.steps)
     clocks = sampler.stop() if rank == 0 else None
     ms_per_step = ms / args.steps
+    if args.dump_outputs and rank == 0:
+        # what the last timed step computed: every projection's output and the logits, fp32 (fixed seeds: identical inputs
+        # in every run); ~6 MB for Llama-3.1-8B
+        dump_outputs(args.dump_outputs, tok.outputs())
 
     # ---- the same token with the reference's Llama launch list (q, k+v as two calls), same run, same weights ----
     ref_list = None
@@ -680,9 +683,6 @@ def run_gpu_arm(args, cfg):
 
     peak, peak_src = read_peaks()
     achieved = tok.alg_bytes / (ms_per_step * 1e-3) / 1e9          # per rank (each rank streams its own shard)
-    # DRAM traffic of the dominant kernel from the committed ncu capture (profiles/): measured bytes / algorithmic bytes
-    # of the captured launch, applied to the average launch of this step
-    traffic = ncu_traffic_per_launch(tok)
     cpu_baseline = None
     check = None
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
@@ -733,12 +733,8 @@ def run_gpu_arm(args, cfg):
                        "row_parallel_sum": ("fused into the GEMM epilogue over NVLink peer memory" if tok.fused_reduce else
                                             ("NCCL all-reduce per row-parallel output" if world > 1 else "none (single GPU)"))},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": peak_src, "kernel": "gemm_tc_i8_kernel (tcgen05 kind::i8 decode-GEMM)",
-                         "note": "achieved = algorithmic bytes of the step / step time = average over the step's launches of the "
-                                 "dominant kernel (it is 100 % of the launches, profiles/r02_launches.md); traffic = bytes per average "
-                                 "launch scaled from this round's ncu --set full capture of the kernel on the gate shape "
-                                 "(profiles/r02_ncu_gate.csv: 29.486 MB read for 29.46 MB algorithmic, ratio 1.001; q and lm_head "
-                                 "captures beside it)"},
+                         "peak_source": peak_src, "kernel": "gemm_tc_i8_kernel (wgmma u8 x s8 decode-GEMM)",
+                         "note": "achieved = algorithmic bytes of the step / step time"},
             "cpu_baseline": cpu_baseline,
             "e2e": {"value": 1000.0 / e2e_ms, "unit": "tok/s", "h2d_bytes_per_step": hx.numel() * 2,
                     "d2h_bytes_per_step": hlogits.numel() * hlogits.element_size(),
@@ -777,12 +773,14 @@ def main():
     ap.add_argument("--no-fuse", action="store_true", help="one launch per projection (no exl3_mgemm for k+v / gate+up)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-qgemm", action="store_true", help="skip the per-shape qgemm GB/s + prefill tensor-pipe section (N = 1 only)")
-    ap.add_argument("--fused-allreduce", action="store_true", help="(default for N > 1 since round 2; kept for old command lines)")
+    ap.add_argument("--fused-allreduce", action="store_true", help="(the default for N > 1; kept for old command lines)")
     ap.add_argument("--nccl-allreduce", action="store_true",
                     help="N > 1: row-parallel outputs as exl3_gemm + NCCL all-reduce (what the reference issues) instead of the one-kernel "
                          "exl3_gemm_allreduce")
     ap.add_argument("--tp-shapes", type=int, default=0, help="debug: run rank 0's shard shapes of a TP-N token on one GPU without the all-reduce")
     ap.add_argument("--cpu-budget", type=float, default=0.0, help="seconds; 0 = the fixed sample (all of layer 0)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed (every projection's output, the logits) as DIR/<name>.npy, float32")
     args = ap.parse_args()
     cfg = MODELS[args.model]
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 """
-exllamav3_b200 -- Blackwell-native (sm_100a) EXL3 quantized-GEMM path.
+exllamav3_b200 -- Hopper-native (sm_90a) EXL3 quantized-GEMM path.
 
     ext           reference-named operator surface (exl3_gemm, exl3_mgemm, reconstruct*, had_r_128, hgemm,
                   BC_LinearEXL3) over the C ABI of libexl3b200.so -- the drop-in boundary

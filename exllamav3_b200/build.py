@@ -1,5 +1,5 @@
 """
-In-tree build of libexl3b200.so (hand-written sm_100a kernels + C ABI) with nvcc.  No torch headers are involved:
+In-tree build of libexl3b200.so (hand-written sm_90a kernels + C ABI) with nvcc.  No torch headers are involved:
 the library is plain CUDA C++ behind the C ABI in include/exl3b200.h.
 
     python -m exllamav3_b200.build [-f] [-v]
@@ -22,7 +22,7 @@ HEADERS = ["common.cuh", "decode.cuh", "epilogue.cuh", "ptx.cuh", "tc_common.cuh
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
 ]
@@ -30,7 +30,7 @@ if os.environ.get("EXL3B_TC_DEBUG", "0") != "0":       # bring-up build: in-kern
     NVCC_FLAGS.append("-DEXL3B_TC_DEBUG")
 
 
-if os.environ.get("EXL3B_NVCC_EXTRA"):                   # experiment switches, e.g. EXL3B_NVCC_EXTRA="-DEXL3B_I8_K4_BRANCHFREE=1" (+ -f)
+if os.environ.get("EXL3B_NVCC_EXTRA"):                   # extra nvcc flags, e.g. EXL3B_NVCC_EXTRA="-Xptxas -warn-spills" (+ -f)
     NVCC_FLAGS += os.environ["EXL3B_NVCC_EXTRA"].split()
 
 

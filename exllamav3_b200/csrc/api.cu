@@ -49,8 +49,8 @@ int get_ctx(DevCtx** out)
     {
         cudaDeviceProp prop;
         EXL3B_CUDA(cudaGetDeviceProperties(&prop, dev));
-        EXL3B_CHECK(prop.major == 10, EXL3B_ERR_CUDA,
-                    "exl3b200 is built for sm_100a only; device %d is sm_%d%d (no fallback path exists)",
+        EXL3B_CHECK(prop.major == 9 && prop.minor == 0, EXL3B_ERR_CUDA,
+                    "exl3b200 is built for sm_90a only; device %d is sm_%d%d (no fallback path exists)",
                     dev, prop.major, prop.minor);
         c.num_sms = prop.multiProcessorCount;
         c.cc = prop.major * 10 + prop.minor;
@@ -61,7 +61,7 @@ int get_ctx(DevCtx** out)
         EXL3B_CUDA(cudaMalloc(&c.tmap_slots, (size_t) DevCtx::NUM_SLOTS * DevCtx::TMAP_SLOTS * 128));
         EXL3B_CUDA(cudaMalloc(&c.i8_parts, (size_t) DevCtx::NUM_SLOTS * DevCtx::I8_PART_CTAS * 1024 * sizeof(float)));
         EXL3B_CUDA(cudaMemset(c.i8_parts, 0xff, (size_t) DevCtx::NUM_SLOTS * DevCtx::I8_PART_CTAS * 1024 * sizeof(float)));
-        // tiled / plain transformed activations: one pass of the exact tcgen05 path is <= 256 rows (gemm_tc.cu)
+        // tiled / plain transformed activations: one pass of the exact path is <= 128 rows (gemm_tc.cu); sized for 256
         c.xh_tiled_slot_bytes = (size_t) 2 * 256 * DevCtx::XH_MAX_K;
         EXL3B_CUDA(cudaMalloc(&c.xh_tiled, c.xh_tiled_slot_bytes * DevCtx::XH_SLOTS));
         EXL3B_CUDA(cudaMemset(c.xh_tiled, 0, c.xh_tiled_slot_bytes * DevCtx::XH_SLOTS));
@@ -99,7 +99,7 @@ int ensure_xh_tiled(DevCtx* ctx, size_t bytes_per_slot)
 
 }  // namespace exl3b
 
-namespace exl3b { void tc_set_debug_buffer(unsigned long long* d); void tc_set_knob(int k); void hgemm_set_pair_mode(int mode); }
+namespace exl3b { void tc_set_debug_buffer(unsigned long long* d); void tc_set_knob(int k); }
 using namespace exl3b;
 
 extern "C" {
@@ -112,11 +112,9 @@ int64_t exl3b_launch_count(void) { return g_launches.load(); }
 
 int exl3b_set_gemm_path(int tag) { return g_force_path.exchange(tag); }
 
-// bring-up aid (not in the public header): per-CTA %globaltimer stamps of the tcgen05 kernel, 16 x u64 per CTA
+// bring-up aid (not in the public header): per-CTA %globaltimer stamps of the tensor-core kernels, 16 x u64 per CTA
 void exl3b_debug_tc_timeline(void* dev_buf) { exl3b::tc_set_debug_buffer((unsigned long long*) dev_buf); }
 void exl3b_debug_tc_knob(int knob) { exl3b::tc_set_knob(knob); }
-// measurement aid (not in the public header): dense GEMM tile mode, 0 = auto (CTA pairs above 128 rows), 1 = single CTA, 2 = pairs
-void exl3b_debug_hgemm_pair(int mode) { exl3b::hgemm_set_pair_mode(mode); }
 void exl3b_debug_reconstruct_had(int mode) { exl3b::reconstruct_had_set_mode(mode); }
 
 int exl3b_num_sms(int device)
@@ -190,18 +188,18 @@ int exl3b_reconstruct_had(void* stream, void* unpacked, const void* packed, cons
 }
 
 // Path selection: auto = int8 tensor-core codebook path for mul1 at m <= 4 (like the reference, whose default for mul1 at
-// m <= 2 is its int8 GEMV, exl3_gemm.cu:182-186), else the bit-exact tcgen05 path; exl3b_set_gemm_path overrides.
-// Rows 5..8 exist on the int8 path (forced) but are not selected automatically yet: its per-unit digit warps are the
-// pacing role there (measured 25 us vs 19 us for the exact path on 4096 x 4096 at m = 8).
+// m <= 2 is its int8 GEMV, exl3_gemm.cu:182-186), else the bit-exact tensor-core path; exl3b_set_gemm_path overrides.
+// Rows 5..8 exist on the int8 path (forced) but are not selected automatically: its two per-unit digit warps quantise
+// every row of every unit, a cost that grows with m while the exact path's per-unit work does not.
 static int select_gemm_path(const GemmArgs& g, int force_shape_idx = -1)
 {
     int path = g_force_path.load();
     if (path == EXL3B_TAG_TC_I8_ROUTED) path = 0;            // only concerns exl3b_mgemm
     // per-call kernel choice, the role of the reference's force_shape_idx (exl3_gemm.cuh:28; science/qgemm_benchmark.py times
-    // every "shape" 1..exl3_gemm_num_kernel_shapes() this way): 1 = CUDA-core twin, 2 = exact tcgen05 kernel; <= 0 = automatic
+    // every "shape" 1..exl3_gemm_num_kernel_shapes() this way): 1 = CUDA-core twin, 2 = exact tensor-core kernel; <= 0 = automatic
     if (force_shape_idx > 0)
     {
-        EXL3B_CHECK(force_shape_idx <= 2, EXL3B_ERR_ARG, "exl3_gemm: force_shape_idx %d out of range (1 = CUDA-core, 2 = tcgen05)", force_shape_idx);
+        EXL3B_CHECK(force_shape_idx <= 2, EXL3B_ERR_ARG, "exl3_gemm: force_shape_idx %d out of range (1 = CUDA-core, 2 = tensor-core)", force_shape_idx);
         path = force_shape_idx == 1 ? EXL3B_TAG_SIMT : EXL3B_TAG_TC;
     }
     if (path == EXL3B_TAG_TC_I8_CHAIN)
@@ -212,7 +210,7 @@ static int select_gemm_path(const GemmArgs& g, int force_shape_idx = -1)
     if (path == EXL3B_TAG_TC_I8)
         EXL3B_CHECK(gemm_tc_i8_supported(g), EXL3B_ERR_UNSUPPORTED, "exl3_gemm: int8 tensor-core path forced but unsupported (needs mul1, m <= 4, or m <= 8 with m * k <= 32768)");
     if (path == EXL3B_TAG_TC)
-        EXL3B_CHECK(gemm_tc_supported(g), EXL3B_ERR_UNSUPPORTED, "exl3_gemm: tcgen05 path forced but shape unsupported");
+        EXL3B_CHECK(gemm_tc_supported(g), EXL3B_ERR_UNSUPPORTED, "exl3_gemm: tensor-core path forced but shape unsupported");
     if ((path == EXL3B_TAG_TC_I8 || (path == 0 && g.m <= 4)) && gemm_tc_i8_supported(g)) return EXL3B_TAG_TC_I8;
     if (path != EXL3B_TAG_SIMT && gemm_tc_supported(g)) return EXL3B_TAG_TC;
     return EXL3B_TAG_SIMT;
@@ -234,11 +232,11 @@ int exl3b_gemm_plan(int m, int k, int n, int K, int cb, int num_sms, int force_n
     out->path = path;
     if (path == EXL3B_TAG_SIMT) return 0;
     TcPlan pl{};
-    const int m_pass = path == EXL3B_TAG_TC && m > 256 ? 256 : m;
+    const int m_pass = path == EXL3B_TAG_TC && m > 128 ? 128 : m;
     r = path == EXL3B_TAG_TC_I8 ? plan_gemm_tc_i8(m, k, n, K, num_sms, g.max_ctas, &pl)
                                 : plan_gemm_tc(m_pass, k, n, K, num_sms, g.max_ctas, &pl);
     if (r) return r;
-    out->passes = path == EXL3B_TAG_TC ? (m + 255) / 256 : 1;
+    out->passes = path == EXL3B_TAG_TC ? (m + 127) / 128 : 1;
     out->rows = pl.rows; out->grid = pl.grid; out->stages = pl.stages; out->smem_bytes = pl.smem_total;
     out->a_stages = pl.a_stages; out->d_bufs = pl.d_bufs; out->tmem_cols = pl.tmem_cols; out->units = pl.units;
     return 0;
@@ -262,7 +260,7 @@ int exl3b_gemm(void* stream_, const void* A, const void* B, void* C, const void*
 {
     cudaStream_t stream = (cudaStream_t) stream_;
     int r = check_kcb(K, cb); if (r) return r;
-    EXL3B_CHECK(force_shape_idx <= 2, EXL3B_ERR_ARG, "exl3_gemm: force_shape_idx %d out of range (1 = CUDA-core, 2 = tcgen05)", force_shape_idx);
+    EXL3B_CHECK(force_shape_idx <= 2, EXL3B_ERR_ARG, "exl3_gemm: force_shape_idx %d out of range (1 = CUDA-core, 2 = tensor-core)", force_shape_idx);
     EXL3B_CHECK(m >= 0 && k >= 0 && n >= 0, EXL3B_ERR_SHAPE, "exl3_gemm: negative size");
     EXL3B_CHECK(k % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm: k (%d) must be divisible by 128", k);
     EXL3B_CHECK(n % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm: n (%d) must be divisible by 128", n);
@@ -388,7 +386,7 @@ int exl3b_mgemm(void* stream, const void* A, const uint64_t* B_ptrs, void* C, co
     if ((path == EXL3B_TAG_TC_I8 || path == EXL3B_TAG_TC_I8_ROUTED || (path == 0 && m <= 4)) && mgemm_tc_i8_supported(ctx, a))
         return launch_mgemm_tc_i8((cudaStream_t) stream, ctx, a);
     // routed / weighted calls (MoE decode: indices, weights, expert-range filter) with mul1 at <= 4 rows: the tensor-core
-    // kernel with one CTA group per active slot (verified on hardware in round 2; EXL3B_TAG_SIMT still forces the CUDA-core twin)
+    // kernel with one CTA group per active slot (EXL3B_TAG_SIMT still forces the CUDA-core twin)
     if ((path == 0 || path == EXL3B_TAG_TC_I8 || path == EXL3B_TAG_TC_I8_ROUTED) && (a.indices || a.weights || a.min_index >= 0)
         && mgemm_tc_i8_routed_supported(ctx, a))
         return launch_mgemm_tc_i8_routed((cudaStream_t) stream, ctx, a);

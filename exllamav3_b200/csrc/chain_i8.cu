@@ -3,8 +3,8 @@
 // (gate + up -> silu * mul -> down: what the reference's BC_GatedMLP issues as three launches, libtorch/mlp.cpp:14-91; the
 // projections of BC_Attention, libtorch/attention.cpp:286-365) -- with the weight stream never stopping at a GEMM boundary.
 //
-// Arithmetic per weight is that of gemm_tc_i8_body.cuh (the product word state * 0x83DCD12D written to TMEM as four u8
-// K-elements of a tcgen05.mma.kind::i8 operand, activations as balanced 16-bit integers in two int8 digits); what is new:
+// Arithmetic per weight is that of gemm_tc_i8_body.cuh (the product word state * 0x83DCD12D as four u8 K-elements of a
+// register A operand of wgmma, activations as balanced 16-bit integers in two int8 digits); what is new:
 //
 //   * ops and stages.  The list is cut into STAGES; the ops of a stage are independent (same or external inputs) and
 //     their 128 x 128 units form one stream-K unit space over the persistent grid; a stage's inputs may be outputs of
@@ -12,11 +12,8 @@
 //     a global counter, and only the warps that PREPARE activations wait for it.  The TMA producer and the decode warps
 //     run on into the next stage's weights (they depend on no activation), so HBM streams through the boundary and the
 //     first operand stages of the next GEMM are decoded before its input exists.
-//   * the unit pipeline itself is the one of gemm_tc_i8_body.cuh (two decode groups of eight warps, three 128-column TMEM
-//     operand stages, one MMA issuer).  A finer-grained variant -- four quads of four warps issuing their own MMAs from
-//     32-column slots -- was built and measured first (round 2, profiles/r02_chain_notes.md): 1.2 us per unit against 0.5,
-//     because every handshake (mbarrier round trip, tcgen05.wait::st, fence) costs 100-300 cycles of latency regardless of
-//     how little work it guards, so halving the work per round doubled the stall time per weight.
+//   * the unit pipeline itself is the one of gemm_tc_i8_body.cuh (two decode groups of two warpgroups, each warpgroup
+//     decoding its weights straight into wgmma A fragments and accumulating in registers).
 //   * activation scale without a Hadamard pass.  The quantisation scale only needs an upper bound of max |xh| over
 //     the row; xh is a block-orthonormal transform of x * suh, so max_kb || (x * suh)_kb ||_2 is one -- a plain
 //     reduction pass over the row by three warps (which also applies silu * mul for the gated-MLP input and caches
@@ -25,8 +22,8 @@
 //     (|q| <= 32512 still holds; the scale is up to ~3x larger than the exact maximum, i.e. activations carry ~14.5
 //     instead of 16 bits: rel-RMS contribution 1e-4, tolerance tests in tests/test_chain.py.)
 //
-// Roles (768 threads): warp 0 TMA producer, warp 1 MMA issuer, warps 2-3 activation / digit warps, warps 4-19 decode (two
-// groups of eight), warps 20-23 epilogue.  TMEM: 3 operand stages x 128 columns + 2 accumulators x 16 columns.
+// Roles (768 threads): warp 0 TMA producer, warp 1 idle, warps 2-3 activation / digit warps, warps 4-19 decode + MMA (two
+// groups of two warpgroups), warps 20-23 epilogue; accumulators reach the epilogue through two shared-memory buffers.
 #include "tc_common.cuh"
 #include "i8_math.cuh"
 #include <mutex>
@@ -37,13 +34,10 @@ namespace exl3b {
 using namespace ptx;
 
 constexpr int CH_THREADS = 768;
-constexpr int CH_MMA_WARP = 1;
 constexpr int CH_XF_WARP0 = 2, CH_XF_WARPS = 2;
 constexpr int CH_DEC_WARP0 = 4, CH_DEC_WARPS = 16, CH_DEC_GROUPS = 2;
 constexpr int CH_EPI_WARP0 = 20;
-constexpr int CH_A_STAGES = 3, CH_A_STAGE_COLS = 128;
-constexpr int CH_D_COL0 = CH_A_STAGES * CH_A_STAGE_COLS;               // 384
-constexpr int CH_NT = 16, CH_MR = 4;
+constexpr int CH_MR = 4;
 constexpr int CH_B_BYTES = 4096, CH_B_STAGE = 4096 + 64;               // digit tile + per-row digit sums
 constexpr int CH_SUB_UNITS = 96;                                       // int32 accumulator safety (see I8_SUB_UNITS)
 constexpr int CH_MAX_STAGES = 16;
@@ -83,7 +77,10 @@ struct ChainParams
     CUtensorMap tmaps_inline[CH_MAX_INLINE];
 };
 
-struct ChainSmem { int off_b, off_tile, off_bars, off_cache, off_suh, total; };
+// accumulator hand-off decode groups -> epilogue: [2 buffers][2 groups][128 columns][2 CH_MR] int32, then [2][2][8] digit sums
+constexpr int CH_D_BYTES = 2 * 2 * 128 * 2 * CH_MR * 4 + 2 * 2 * 8 * 4;
+
+struct ChainSmem { int off_b, off_tile, off_bars, off_d, off_cache, off_suh, total; };
 
 __host__ __device__ inline ChainSmem chain_smem(int S, int w_bytes, int cache_bytes, int suh_bytes)
 {
@@ -92,7 +89,8 @@ __host__ __device__ inline ChainSmem chain_smem(int S, int w_bytes, int cache_by
     L.off_tile = L.off_b + S * CH_B_STAGE;
     L.off_tile = (L.off_tile + 127) & ~127;
     L.off_bars = L.off_tile + CH_MR * 128 * 4;
-    L.off_cache = L.off_bars + 2048;
+    L.off_d = L.off_bars + 2048;
+    L.off_cache = L.off_d + CH_D_BYTES;
     L.off_suh = L.off_cache + cache_bytes;
     L.total = L.off_suh + suh_bytes;
     return L;
@@ -170,14 +168,11 @@ struct ChainCtx
     uint32_t bar0;
     int S, w_bytes;
     ChainSmem L;
-    uint32_t tmem_base;
     unsigned long long* dbg;
     int trace_seq;            // bring-up: the unit (CTA-local index) whose steps are stamped
     __device__ __forceinline__ uint32_t W_FULL(int s) const { return bar0 + 8u * s; }
     __device__ __forceinline__ uint32_t W_EMPTY(int s) const { return bar0 + 8u * (CH_MAX_STAGES + s); }
     __device__ __forceinline__ uint32_t X_FULL(int s) const { return bar0 + 8u * (2 * CH_MAX_STAGES + s); }
-    __device__ __forceinline__ uint32_t A_FULL(int a) const { return bar0 + 8u * (3 * CH_MAX_STAGES + a); }
-    __device__ __forceinline__ uint32_t A_EMPTY(int a) const { return bar0 + 8u * (3 * CH_MAX_STAGES + 4 + a); }
     __device__ __forceinline__ uint32_t D_FULL(int b) const { return bar0 + 8u * (3 * CH_MAX_STAGES + 8 + b); }
     __device__ __forceinline__ uint32_t D_EMPTY(int b) const { return bar0 + 8u * (3 * CH_MAX_STAGES + 10 + b); }
     __device__ __forceinline__ uint32_t IN_BAR() const { return bar0 + 8u * (3 * CH_MAX_STAGES + 12); }
@@ -190,42 +185,47 @@ constexpr int CH_NUM_BARS = 3 * CH_MAX_STAGES + 13;                    // 61 bar
 #define CH_STAMP(cond, slot) do { } while (0)
 #endif
 
-// One unit (128 k x 128 n weights) of a decode group (8 warps: two per TMEM lane quarter, alternate k-tiles): the pipeline of
-// gemm_tc_i8_body.cuh -- weight words from the ring stage, four tiles per warp into the unit's 128-column operand stage.
+// One unit (128 k x 128 n weights) of a decode warpgroup: the pipeline of gemm_tc_i8_body.cuh -- weight words from the ring
+// stage, the warp's tile column of k-tiles c and 4 + c decoded straight into wgmma A fragments, 16 MMAs into acc.
 template <int K>
-__device__ __forceinline__ void group_unit(const ChainCtx& cx, int q, int sub, int lane, int s, int sph, int as, int aph,
+__device__ __forceinline__ void group_unit(const ChainCtx& cx, int tl, int lane, int s, int sph, int m, uint32_t (&acc)[CH_MR], int& tsum,
                                            [[maybe_unused]] bool trace)
 {
-    const int tl = strip_tile(q, lane), chunk = lane & 7;
-    const int prev_lane = (lane & ~7) | ((lane + 7) & 7);
-    const uint32_t lane_base = (uint32_t) (q * 32) << 16;
-    [[maybe_unused]] const bool tr = trace && q == 0 && sub == 0 && lane == 0;
+    const int chunk = lane >> 2, c = lane & 3;
+    [[maybe_unused]] const bool tr = trace && tl == 0 && lane == 0;
     CH_STAMP(tr, 0);
     mbar_wait<32>(cx.W_FULL(s), sph);
     CH_STAMP(tr, 1);
     const uint32_t* wst = reinterpret_cast<const uint32_t*>(cx.smem + s * cx.w_bytes);
-    uint32_t w[4][K + 1];
-    tc_load_tiles4<K>(wst, tl, chunk, prev_lane, sub, 2, w);           // tiles sub, sub + 2, sub + 4, sub + 6
-    CH_STAMP(tr, 2);
-    mbar_wait(cx.A_EMPTY(as), aph ^ 1);
-    tc_fence_after();
-    CH_STAMP(tr, 3);
+    uint32_t w[2][K + 1];
     #pragma unroll
-    for (int j = 0; j < 4; ++j)
+    for (int r = 0; r < 2; ++r) load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, w[r]);
+    mbar_wait(cx.X_FULL(s), sph);                                      // the unit's activation digits
+    CH_STAMP(tr, 2);
+    if (c < m) tsum += *reinterpret_cast<const int*>(cx.smem + cx.L.off_b + s * CH_B_STAGE + CH_B_BYTES + 4 * c);
+    const uint64_t desc_s = smem_desc(smem_u32(cx.smem + cx.L.off_b + s * CH_B_STAGE), 128, 4096, 0);
+    #pragma unroll
+    for (int r = 0; r < 2; ++r)
     {
-        const int t = sub + 2 * j;
-        uint32_t o[16];
-        if (q & 1) decode16_i8<K, 1>(w[j], o); else decode16_i8<K, 0>(w[j], o);
-        tmem_st_32x32b_x16(cx.tmem_base + lane_base + as * CH_A_STAGE_COLS + 16 * t, o);
+        uint32_t o0[16], o1[16];
+        decode16_i8<K, 0>(w[r], o0);
+        decode16_i8<K, 1>(w[r], o1);
+        #pragma unroll
+        for (int i = 0; i < CH_MR; ++i) reg_fence(acc[i]);
+        wgmma_fence();
+        #pragma unroll
+        for (int j = 0; j < 8; ++j)
+            wgmma_u8s8_n8(acc, o0[2 * j], o1[2 * j], o0[2 * j + 1], o1[2 * j + 1], desc_s + (uint64_t) (16 * (8 * r + j)));
+        wgmma_commit();
+        wgmma_wait<0>();
+        #pragma unroll
+        for (int i = 0; i < 16; ++i) { reg_fence(o0[i]); reg_fence(o1[i]); }
+        #pragma unroll
+        for (int i = 0; i < CH_MR; ++i) reg_fence(acc[i]);
     }
-    CH_STAMP(tr, 4);
-    tc_wait_st();
-    CH_STAMP(tr, 5);
-    tc_fence_before();
-    if (sub == 0 && q == 0) mbar_wait(cx.X_FULL(s), sph);              // the group's lead warp vouches for the activation digits
+    CH_STAMP(tr, 3);
     __syncwarp();
-    if (lane == 0) { mbar_arrive(cx.A_FULL(as)); mbar_arrive(cx.W_EMPTY(s)); }
-    CH_STAMP(tr, 6);
+    if (lane == 0) mbar_arrive(cx.W_EMPTY(s));
 }
 
 __device__ __forceinline__ void ch_watchdog(uint32_t& polls, unsigned long long& t0, const char* what, int a, int b)
@@ -257,10 +257,11 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
     CH_STAMP(threadIdx.x == 0, 61);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + cx.L.off_bars);
     cx.bar0 = smem_u32(bars);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + cx.L.off_bars + 8 * CH_NUM_BARS);
-    unsigned int* s_norm2 = reinterpret_cast<unsigned int*>(tmem_slot + 4);                                  // [MR] float bits
-    int* s_tout = reinterpret_cast<int*>(tmem_slot + 8);                                                     // [2][MR]
-    float* s_scale = reinterpret_cast<float*>(tmem_slot + 8 + 8);                                            // [CH_SCALE_SLOTS][MR]
+    uint32_t* misc = reinterpret_cast<uint32_t*>(smem + cx.L.off_bars + 8 * CH_NUM_BARS);
+    unsigned int* s_norm2 = reinterpret_cast<unsigned int*>(misc + 4);                                       // [MR] float bits
+    float* s_scale = reinterpret_cast<float*>(misc + 8 + 8);                                                 // [CH_SCALE_SLOTS][MR]
+    int32_t* s_d = reinterpret_cast<int32_t*>(smem + cx.L.off_d);                                            // [dbuf][group][128][2 MR]
+    int* s_dt = reinterpret_cast<int*>(smem + cx.L.off_d + CH_D_BYTES - 2 * 2 * 8 * 4);                     // [dbuf][group][8]
     half* cache = reinterpret_cast<half*>(smem + cx.L.off_cache);
     half* suh_s = reinterpret_cast<half*>(smem + cx.L.off_suh);
 
@@ -270,19 +271,15 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
         for (int i = lane; i < CH_NUM_BARS; i += 32)
         {
             int cnt = 1;
-            if (i >= CH_MAX_STAGES && i < 2 * CH_MAX_STAGES) cnt = CH_DEC_WARPS / CH_DEC_GROUPS + 1;     // W_EMPTY: the group's warps + MMA completion
-            else if (i >= 3 * CH_MAX_STAGES && i < 3 * CH_MAX_STAGES + 4) cnt = CH_DEC_WARPS / CH_DEC_GROUPS;   // A_FULL
+            if (i >= CH_MAX_STAGES && i < 2 * CH_MAX_STAGES) cnt = CH_DEC_WARPS / CH_DEC_GROUPS;         // W_EMPTY: the group's warps, after their MMAs
+            else if (i >= 3 * CH_MAX_STAGES + 8 && i < 3 * CH_MAX_STAGES + 10) cnt = CH_DEC_WARPS;         // D_FULL: every decode warp
             else if (i >= 3 * CH_MAX_STAGES + 10 && i < 3 * CH_MAX_STAGES + 12) cnt = 4;                 // D_EMPTY: the 4 epilogue warps
             else if (i == 3 * CH_MAX_STAGES + 12) cnt = 2;                                               // IN_BAR: suh copy + input copy
             mbar_init(cx.bar0 + 8u * i, cnt);
         }
         fence_barrier_init();
-        tmem_alloc<512>(smem_u32(tmem_slot));
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    cx.tmem_base = *tmem_slot;
 
     const int cta = blockIdx.x, G = gridDim.x;
 
@@ -313,66 +310,7 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
         }
         __syncwarp();
     }
-    else if (warp == CH_MMA_WARP)
-    {
-        // =========================== MMA issuer ===========================
-        const uint32_t idesc = idesc_u8s8_s32(128, CH_NT);
-        const uint32_t tb = __shfl_sync(0xffffffffu, cx.tmem_base, 0);
-        const uint64_t desc0 = smem_desc(smem_u32(smem + cx.L.off_b), 128, 4096, 0);
-        const uint32_t desc_hi = (uint32_t) (desc0 >> 32), desc_lo0 = (uint32_t) desc0;
-        uint32_t desc_lo = desc_lo0;
-        Cursor c; c.init(ops, stages, p.n_stages, cta, G);
-        int s = 0, as = 0, aph = 0, dbuf = 0, dphase = 0, tsum = 0, cur_op = -1, m = 0;
-        uint32_t acc = 0;
-        while (c.valid)
-        {
-            int sb, se; c.sub_bounds(sb, se);
-            const bool first = c.seq == sb, last = c.seq == se - 1;
-            if (c.op != cur_op) { cur_op = c.op; m = ops[cur_op].m; }
-            if (first)
-            {
-                mbar_wait(cx.D_EMPTY(dbuf), dphase ^ 1);               // the epilogue has drained this accumulator
-                acc = 0; tsum = 0;
-            }
-            CH_STAMP(lane == 0 && c.seq == cx.trace_seq, 8);
-            // (the unit's activation digits are complete too: the decode group's lead warp waited for X_FULL before it arrived)
-            mbar_wait(cx.A_FULL(as), aph);
-            tc_fence_after();
-            CH_STAMP(lane == 0 && c.seq == cx.trace_seq, 9);
-            if (lane < m) tsum += *reinterpret_cast<const int*>(smem + cx.L.off_b + s * CH_B_STAGE + CH_B_BYTES + 4 * lane);
-            if (last)
-            {
-                if (lane < m) s_tout[dbuf * CH_MR + lane] = tsum;      // visible to the epilogue before D_FULL fires
-                __threadfence_block();
-                __syncwarp();
-            }
-            if (elect_one())
-            {
-                const uint32_t d_addr = tb + CH_D_COL0 + dbuf * CH_NT;
-                uint32_t a_addr = tb + as * CH_A_STAGE_COLS;
-                uint32_t dl = desc_lo;
-                #pragma unroll
-                for (int j = 0; j < 16; ++j)
-                {
-                    mma_i8_ts_step<8, 16>(d_addr, a_addr, dl, desc_hi, idesc, acc);
-                    acc = 1;
-                }
-                tc_commit(cx.A_EMPTY(as));
-                tc_commit(cx.W_EMPTY(s));
-                if (last) tc_commit(cx.D_FULL(dbuf));
-            }
-            acc = 1;
-            __syncwarp();
-            CH_STAMP(lane == 0 && c.seq == cx.trace_seq, 10);
-            if (last) { dbuf ^= 1; if (dbuf == 0) dphase ^= 1; }
-            desc_lo += CH_B_STAGE >> 4;
-            if (++s == S) { s = 0; desc_lo = desc_lo0; }
-            if (++as == CH_A_STAGES) { as = 0; aph ^= 1; }
-            c.next();
-        }
-        __syncwarp();
-    }
-    else if (warp < CH_DEC_WARP0)
+    else if (warp >= CH_XF_WARP0 && warp < CH_DEC_WARP0)
     {
         // =========================== activation warps: scale pass per op, digits per unit ===========================
         const int xw = warp - CH_XF_WARP0;
@@ -384,8 +322,7 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
         #pragma unroll
         for (int r = 0; r < CH_MR; ++r) inv_scale[r] = 0.f;
         // the op's fields live in registers: `ops` is a generic pointer (kernel parameters or global memory), and every
-        // shared-memory store in the loops below would otherwise force a reload of each field (measured: 6 us per scale pass
-        // and 1 us per unit of digits with the fields read through the pointer)
+        // shared-memory store in the loops below would otherwise force a reload of each field
         struct { const void* A; const void* A2; const half* suh; int m, k, KB, in_mode, cached, suh_cached, stage; } o{};
         while (c.valid)
         {
@@ -581,9 +518,15 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                         i8_digits(v1, inv_scale[r], qs, hi_w[1], lo_w[1]);
                         i8_digits(v2, inv_scale[r], qs, hi_w[2], lo_w[2]);
                         i8_digits(v3, inv_scale[r], qs, hi_w[3], lo_w[3]);
-                        uint8_t* drow = dst + (lane * 8 + 2 * r) * 16;
-                        *reinterpret_cast<uint4*>(drow) = make_uint4(hi_w[0], hi_w[1], hi_w[2], hi_w[3]);
-                        *reinterpret_cast<uint4*>(drow + 16) = make_uint4(lo_w[0], lo_w[1], lo_w[2], lo_w[3]);
+                        // K order of the wgmma fragments (gemm_tc_i8_body.cuh): k = 4 lane + e -> K-chunk 16 (lane / 16) + 4 (lane % 4) + e,
+                        // byte 4 ((lane / 4) % 4)
+                        uint8_t* drow = dst + ((16 * (lane >> 4) + 4 * (lane & 3)) * 8 + 2 * r) * 16 + 4 * ((lane >> 2) & 3);
+                        #pragma unroll
+                        for (int e = 0; e < 4; ++e)
+                        {
+                            *reinterpret_cast<uint32_t*>(drow + e * 128) = hi_w[e];
+                            *reinterpret_cast<uint32_t*>(drow + e * 128 + 16) = lo_w[e];
+                        }
                         qsum[r] = qs;
                     }
                 }
@@ -610,47 +553,66 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
             c.next();
         }
     }
-    else if (warp < CH_EPI_WARP0)
+    else if (warp >= CH_DEC_WARP0 && warp < CH_EPI_WARP0)
     {
-        // =========================== decode groups ===========================
-        const int q = warp & 3, wi = (warp - CH_DEC_WARP0) >> 2;         // wi = 0..3
-        const int g = wi & 1, sub = wi >> 1;
+        // =========================== decode groups: four warpgroups ===========================
+        // warpgroup (g, nh): units seq = g (mod 2), output columns 64 nh .. 64 nh + 63; both groups hand over (possibly zero)
+        // accumulators at every accumulation-chunk boundary, the epilogue adds the two
+        const int wq = warp & 3, wgi = (warp - CH_DEC_WARP0) >> 2;
+        const int g = wgi & 1, nh = wgi >> 1, tl = 4 * nh + wq;
+        const int chunk = lane >> 2, cq = lane & 3;
         Cursor c; c.init(ops, stages, p.n_stages, cta, G);
-        int s = 0, ph = 0, as = 0, aph = 0;
+        int s = 0, ph = 0, dbuf = 0, dphase = 0;
+        uint32_t acc[CH_MR] = {0u, 0u, 0u, 0u};
+        int tsum = 0;
         while (c.valid)
         {
+            int sb, se; c.sub_bounds(sb, se);
+            const bool last = c.seq == se - 1;
             if ((c.seq & 1) == g)
             {
                 const bool trace = c.seq == cx.trace_seq;
-                if constexpr (KSEL != 0) group_unit<KSEL>(cx, q, sub, lane, s, ph, as, aph, trace);
+                const int m = ops[c.op].m;
+                if constexpr (KSEL != 0) group_unit<KSEL>(cx, tl, lane, s, ph, m, acc, tsum, trace);
                 else
                 {
                     switch (ops[c.op].K)
                     {
-                        case 1: group_unit<1>(cx, q, sub, lane, s, ph, as, aph, trace); break;
-                        case 2: group_unit<2>(cx, q, sub, lane, s, ph, as, aph, trace); break;
-                        case 3: group_unit<3>(cx, q, sub, lane, s, ph, as, aph, trace); break;
-                        case 4: group_unit<4>(cx, q, sub, lane, s, ph, as, aph, trace); break;
-                        case 5: group_unit<5>(cx, q, sub, lane, s, ph, as, aph, trace); break;
-                        case 6: group_unit<6>(cx, q, sub, lane, s, ph, as, aph, trace); break;
-                        case 7: group_unit<7>(cx, q, sub, lane, s, ph, as, aph, trace); break;
-                        default: group_unit<8>(cx, q, sub, lane, s, ph, as, aph, trace); break;
+                        case 1: group_unit<1>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
+                        case 2: group_unit<2>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
+                        case 3: group_unit<3>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
+                        case 4: group_unit<4>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
+                        case 5: group_unit<5>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
+                        case 6: group_unit<6>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
+                        case 7: group_unit<7>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
+                        default: group_unit<8>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
                     }
                 }
             }
+            if (last)
+            {
+                mbar_wait(cx.D_EMPTY(dbuf), dphase ^ 1);               // the epilogue has drained this buffer
+                int32_t* dst = s_d + (size_t) ((dbuf * 2 + g) * 128 + 16 * tl + chunk) * (2 * CH_MR);
+                *reinterpret_cast<int2*>(dst + 2 * cq) = make_int2((int) acc[0], (int) acc[1]);
+                *reinterpret_cast<int2*>(dst + 8 * (2 * CH_MR) + 2 * cq) = make_int2((int) acc[2], (int) acc[3]);
+                if (tl == 0 && lane < 4) s_dt[(dbuf * 2 + g) * 8 + cq] = tsum;
+                acc[0] = acc[1] = acc[2] = acc[3] = 0u;
+                tsum = 0;
+                __syncwarp();
+                if (lane == 0) mbar_arrive(cx.D_FULL(dbuf));
+                dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
+            }
             if (++s == S) { s = 0; ph ^= 1; }
-            if (++as == CH_A_STAGES) { as = 0; aph ^= 1; }
             c.next();
         }
     }
-    else
+    else if (warp >= CH_EPI_WARP0)
     {
         // =========================== epilogue ===========================
         pdl_wait();
         const int q = warp & 3;
         const int et = threadIdx.x - CH_EPI_WARP0 * 32;
-        const int col = strip_col(q, lane);
-        const uint32_t lane_base = (uint32_t) (q * 32) << 16;
+        const int col = et;                                             // column of the strip this thread finishes
         float* tile = reinterpret_cast<float*>(smem + cx.L.off_tile);
         auto epi_bar = [] { asm volatile("bar.sync 1, 128;" ::: "memory"); };
         const int part_stride = CH_MR * 128;
@@ -678,21 +640,18 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
             for (int sb = run_begin; sb < run_end; sb += CH_SUB_UNITS)
             {
                 mbar_wait<32>(cx.D_FULL(dbuf), dphase);
-                tc_fence_after();
-                uint32_t rr[16];
-                tmem_ld_32x32b_x16(cx.tmem_base + lane_base + CH_D_COL0 + dbuf * CH_NT, rr);
-                tc_wait_ld();
+                const int32_t* d0 = s_d + (size_t) ((dbuf * 2 + 0) * 128 + col) * (2 * CH_MR);
+                const int32_t* d1 = s_d + (size_t) ((dbuf * 2 + 1) * 128 + col) * (2 * CH_MR);
                 #pragma unroll
                 for (int r = 0; r < CH_MR; ++r)
                 {
                     if (r < o.m)
                     {
-                        const int T = s_tout[dbuf * CH_MR + r];
-                        const long long sp = i8_centred_sum((int) rr[2 * r], (int) rr[2 * r + 1], T);
+                        const int T = s_dt[(dbuf * 2 + 0) * 8 + r] + s_dt[(dbuf * 2 + 1) * 8 + r];
+                        const long long sp = i8_centred_sum(d0[2 * r] + d1[2 * r], d0[2 * r + 1] + d1[2 * r + 1], T);
                         facc[r] += i8_assemble(sp, T, s_scale[(op % CH_SCALE_SLOTS) * CH_MR + r], k_inv, c1);
                     }
                 }
-                tc_fence_before();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(cx.D_EMPTY(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
@@ -785,14 +744,8 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
         }
     }
 
-    tc_fence_before();
     __syncthreads();
     CH_STAMP(threadIdx.x == 0, 62);
-    if (warp == 0)
-    {
-        tc_fence_after();
-        tmem_dealloc<512>(cx.tmem_base);
-    }
     if (threadIdx.x == 0)
     {
         // last CTA out re-zeroes the counters for the next launch (which reads them only after griddepcontrol.wait)
@@ -872,7 +825,7 @@ static int chain_build(const exl3b_chain_op* in, int n_ops, int num_sms, Chain& 
     EXL3B_CHECK(ch.stages.size() <= 255, EXL3B_ERR_UNSUPPORTED, "exl3_chain: more than 255 stages");
     for (const ChainStage& st : ch.stages) if (st.U > Umax) Umax = st.U;
     const int w_bytes = 2048 * Kmax;
-    int S = (220 * 1024 - 128 - CH_MR * 128 * 4 - 2048 - (int) cache - (int) suhb) / (w_bytes + CH_B_STAGE);
+    int S = (220 * 1024 - 128 - CH_MR * 128 * 4 - 2048 - CH_D_BYTES - (int) cache - (int) suhb) / (w_bytes + CH_B_STAGE);
     if (S > CH_MAX_STAGES) S = CH_MAX_STAGES;
     EXL3B_CHECK(S >= 2, EXL3B_ERR_UNSUPPORTED, "exl3_chain: shared-memory budget exceeded");
     const ChainSmem L = chain_smem(S, w_bytes, (int) cache, (int) suhb);

@@ -36,7 +36,7 @@ struct MSlotTable
 struct DevCtx
 {
     static constexpr int NUM_SLOTS = 8;
-    static constexpr size_t WS_BYTES_PER_SLOT = 40u << 20;    // fp32 split-K partials (2 x 148 CTAs x 256 rows x 128 cols)
+    static constexpr size_t WS_BYTES_PER_SLOT = 40u << 20;    // fp32 split-K partials (2 x up to 160 CTAs x 256 rows x 128 cols)
     static constexpr int COUNTERS_PER_SLOT = 32768;
     int device = -1;
     int num_sms = 0;
@@ -46,7 +46,7 @@ struct DevCtx
     MSlotTable* tabs = nullptr;   // NUM_SLOTS mgemm slot tables
     static constexpr int XH_SLOTS = 4;
     static constexpr int XH_MAX_K = 65536;  // largest in_features the fixed activation scratch below is sized for
-    uint8_t* xh_tiled = nullptr;  // XH_SLOTS tiled activation buffers for the tcgen05 path (256 rows x XH_MAX_K fp16 each), allocated once
+    uint8_t* xh_tiled = nullptr;  // XH_SLOTS tiled activation buffers for the tensor-core path (256 rows x XH_MAX_K fp16 each), allocated once
     size_t xh_tiled_slot_bytes = 0;
     half* xh_scratch = nullptr;   // input-transform scratch when the caller passes A_had = NULL (256 x XH_MAX_K), allocated once
     size_t xh_scratch_elems = 0;
@@ -83,7 +83,7 @@ int launch_reconstruct(cudaStream_t stream, half* unpacked, const uint16_t* pack
                        int packed_tiles_n, int K, int cb, int64_t n_offset);
 int launch_reconstruct_had(cudaStream_t stream, half* unpacked, const uint16_t* packed, const half* suh,
                            const half* svh, int k, int n_out, int packed_tiles_n, int K, int cb, int64_t n_offset);
-// tensor-core variant (reconstruct_tc.cu): both Hadamards as tcgen05 GEMMs; the default unless EXL3B_RECONSTRUCT_HAD=simt
+// tensor-core variant (reconstruct_tc.cu): both Hadamards as wgmma GEMMs; the default unless EXL3B_RECONSTRUCT_HAD=simt
 bool reconstruct_had_tc_enabled();
 void reconstruct_had_set_mode(int mode);
 int launch_reconstruct_had_tc(cudaStream_t stream, half* unpacked, const uint16_t* packed, const half* suh, const half* svh,
@@ -102,7 +102,7 @@ struct GemmArgs
     float out_scale;         // extra factor folded into the output transform (mgemm weights), 1.0f otherwise
     int max_ctas;            // 0 = all SMs
 };
-// Launch geometry of one tcgen05 kernel launch: computed by the SAME functions the launchers use (plan_gemm_tc_i8 in
+// Launch geometry of one tensor-core kernel launch: computed by the SAME functions the launchers use (plan_gemm_tc_i8 in
 // gemm_tc_i8.cu, plan_gemm_tc in gemm_tc.cu), pure host arithmetic -- exposed through exl3b_gemm_plan so that the CPU tests
 // can check budgets and the stream-K partition for shapes no GPU test runs.  Returns 0 or a negative status.
 struct TcPlan
@@ -149,7 +149,7 @@ struct MGemmArgs
     const int32_t* size_n_list; const uint64_t* c_ptrs; int num_c_ptrs;
     const int32_t* size_n_host;          // host copy of size_n_list if the caller registered one (exl3b_register_widths), else null
 };
-// fan-out launches (per-matrix widths) on the tcgen05 int8 path: CTA group boundaries proportional to the matrices' unit counts
+// fan-out launches (per-matrix widths) on the wgmma int8 path: CTA group boundaries proportional to the matrices' unit counts
 // (host + tests: the partition the kernel is given); returns the grid size, 0 if the shapes do not fit
 int plan_fanout_groups(int k, const int32_t* widths, int mats, int num_sms, int* cta0 /* mats + 1 */);
 int launch_mgemm(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a);
@@ -164,7 +164,7 @@ int chain_run(cudaStream_t stream, void* chain);
 int chain_destroy(void* chain);
 int launch_mgemm_resolve(cudaStream_t stream, MSlotTable* tab, const MGemmArgs& a, int bszm);
 int launch_mgemm_reduce(cudaStream_t stream, DevCtx* ctx, const MSlotTable* tab, const MGemmArgs& a);
-// routed / weighted exl3_mgemm (MoE decode) on the tcgen05 int8 path (gemm_tc_i8_routed.cu): opt-in, tag EXL3B_TAG_TC_I8_ROUTED
+// routed / weighted exl3_mgemm (MoE decode) on the wgmma int8 path (gemm_tc_i8_routed.cu): opt-in, tag EXL3B_TAG_TC_I8_ROUTED
 bool mgemm_tc_i8_routed_supported(const DevCtx* ctx, const MGemmArgs& a);
 int launch_mgemm_tc_i8_routed(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a);
 

@@ -1,4 +1,4 @@
-// EXL3 trellis decode primitives for sm_100a.
+// EXL3 trellis decode primitives.
 //
 // Format facts (reference: exllamav3_ext/quant/exl3_dq.cuh:15-31, codebook.cuh:56-90, pack.cu:9-57,
 // modules/quant/exl3_lib/quantize.py:22-44):
@@ -12,7 +12,7 @@
 //   (chunk, half) = ONE tile column x 16 k-values from K+1 words (the chunk plus the preceding word), with every
 //   bit offset a compile-time constant.  `half` is warp-uniform in all kernels, so there is no divergence.
 //
-//   Output order matches what a tcgen05 K-major operand row wants: out[j] = packed fp16 pair (k = 2j, 2j+1).
+//   Output order matches what a K-major operand row wants: out[j] = packed fp16 pair (k = 2j, 2j+1).
 #pragma once
 #include <stdint.h>
 #ifndef EXL3B_HOST_EMU
@@ -141,8 +141,8 @@ __device__ __forceinline__ void decode16(const uint32_t (&w)[K + 1], uint32_t (&
 
 // ---- int8 tensor-core codebook path (mul1 only) -----------------------------------------------------------------
 // The mul1 value is k_inv * (1024 + bytesum(state * 0x83DCD12D)) + k_bias (codebook.cuh:77-89).  Instead of summing the
-// four product bytes on the IMAD pipe (IDP.4A shares it, profiles/r01_microbench_pipes.log) the product word itself
-// becomes four unsigned 8-bit K-elements of a tcgen05 kind::i8 operand and the tensor core does the byte sum while
+// four product bytes on the IMAD pipe (IDP.4A shares it) the product word itself
+// becomes four unsigned 8-bit K-elements of a wgmma u8 operand and the tensor core does the byte sum while
 // contracting with the (4x replicated) int8 activation digits.  Cost per weight: window extraction + ONE IMAD.
 // out[k] = state(k) * 0x83DCD12D for the 16 k-rows of the thread's tile column, in k order.
 template <int K, int HALF, int J>

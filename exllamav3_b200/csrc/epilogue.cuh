@@ -1,4 +1,4 @@
-// Output transform shared by the SIMT and tcgen05 GEMM paths.
+// Output transform shared by the SIMT and tensor-core GEMM paths.
 #pragma once
 #include "common.cuh"
 

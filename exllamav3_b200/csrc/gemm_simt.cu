@@ -1,6 +1,6 @@
 // CUDA-core EXL3 GEMM ("SIMT path", tag 100): bring-up / fallback-free correctness path for every (K, cb, m) and the
 // home of the mgemm semantics.  Same thread->column decomposition, split-K protocol and output-transform epilogue as
-// the tcgen05 path (gemm_tc.cu); only the contraction differs (fp32 FMA per thread instead of TMEM/tcgen05).
+// the tensor-core path (gemm_tc.cu); only the contraction differs (fp32 FMA per thread instead of wgmma).
 //
 // Reference behaviour restated: exllamav3_ext/quant/exl3_gemm_kernel.cuh:8-50 (gemm), :88-292 (mgemm),
 // exl3_gemm_inner.cuh:426-480 (output transform), exl3_gemm.cu:341-381 (mgemm semantics).
@@ -292,7 +292,7 @@ __global__ void mgemm_reduce_kernel(void* C, const MSlotTable* tab, int m, int n
     }
 }
 
-// The two bookkeeping stages of exl3_mgemm as stand-alone launches, for the tcgen05 routed path (gemm_tc_i8_routed.cu), which
+// The two bookkeeping stages of exl3_mgemm as stand-alone launches, for the tensor-core routed path (gemm_tc_i8_routed.cu), which
 // replaces only the contraction in between.
 int launch_mgemm_resolve(cudaStream_t stream, MSlotTable* tab, const MGemmArgs& a, int bszm)
 {

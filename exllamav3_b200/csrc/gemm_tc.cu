@@ -1,26 +1,26 @@
-// tcgen05 / TMEM EXL3 decode-GEMM for sm_100a ("TC path", tag 200).
+// wgmma EXL3 decode-GEMM for sm_90a ("TC path", tag 200).
 //
 //   C[m, n] = had128( xh[m, k] @ W_hat[k, n] ) * svh,      xh = fp16( had128(A * suh) / sqrt(128) )
 //
-// Design (see DESIGN.md for the roofline arithmetic):
-//   * swap-AB: the decoded weights are the M = 128 operand of tcgen05.mma (one 128-column strip of W_hat^T), the
-//     activations are the N = 16..256 operand, so the weight stream is decoded exactly ONCE for any m <= 256
+// Design:
+//   * swap-AB: the decoded weights are the M operand of wgmma (one 128-column strip of W_hat^T, two M = 64 halves), the
+//     activations are the N = 16..128 operand, so the weight stream is decoded exactly ONCE for any m <= 128 per pass
 //     (the reference re-streams and re-decodes B per 16-row slab, exl3_gemm_kernel.cuh:37-50).
 //   * persistent stream-K over work units of 128(k) x 128(n) weights: CTA c owns units [U*c/G, U*(c+1)/G), k fastest.
-//   * warp-specialised, 768 threads:
-//        warp 0      producer: cp.async.bulk (TMA engine) of the raw trellis rows + the activation tile into an
-//                    mbarrier ring (weights prefetch starts BEFORE griddepcontrol.wait: PDL overlap with the
-//                    previous kernel's tail)
-//        warp 1      MMA issuer: one elected lane issues tcgen05.mma.kind::f16 with A read from TMEM and B from
-//                    shared memory, accumulators in TMEM; also owns TMEM alloc/dealloc
-//        warps 2-3   (m <= 8) input transform fused in-kernel: A*suh -> 128-point Hadamard -> fp16 core-matrix tile
-//                    written straight into the activation stage (no separate transform launch on the decode path)
-//        warps 4-19  decode: LDS the packed chunk, decode 16 weights per thread per 16x16 tile, tcgen05.st them
-//                    straight into the TMEM A-operand stage (decoded weights never touch shared memory)
-//        warps 20-23 epilogue: tcgen05.ld the accumulators, split-K combine through a global workspace
-//                    (last-arriver reduces in fixed order => deterministic), output Hadamard + svh, store
-//   * activations arrive pre-tiled in the no-swizzle K-major core-matrix layout tcgen05 wants, written by the
-//     input-transform kernel (fused suh scale + 128-point Hadamard), so the B tile is one contiguous bulk copy.
+//   * warp-specialised, 384 threads:
+//        warp 0      producer: TMA of the raw trellis rows + the activation tile into an mbarrier ring (weights prefetch
+//                    starts BEFORE griddepcontrol.wait: PDL overlap with the previous kernel's tail)
+//        warps 2-3   (optional, m <= 8) input transform fused in-kernel: A*suh -> 128-point Hadamard -> fp16 core-matrix tile
+//                    written straight into the activation stage
+//        warpgroups 1-2  decode + MMA + epilogue: warpgroup h owns output columns 64 h .. 64 h + 63 of the strip.  Lane
+//                    (chunk, c) of warp w decodes tile column `chunk` (both halves) of tile 4 h + w for k-tiles c and 4 + c:
+//                    the decoded fp16 pairs ARE the wgmma A fragments (rows chunk / chunk + 8, K pairs c / c + 4), so decoded
+//                    weights never touch shared memory; the K order inside an instruction is permuted accordingly in the
+//                    activation tile.  fp32 accumulators stay in registers over a k-segment, then go through shared memory
+//                    into the split-K combine (global workspace, last arriver reduces in fixed order => deterministic),
+//                    output Hadamard + svh, store.
+//   * activations arrive pre-tiled in the no-swizzle K-major core-matrix layout wgmma reads, written by the input-transform
+//     kernel (fused suh scale + 128-point Hadamard), so the B tile is one contiguous bulk copy.
 //
 // Reference behaviour being replaced: exllamav3_ext/quant/exl3_gemm_kernel.cuh:8-50, exl3_gemm_inner.cuh:22-733.
 #include "common.cuh"
@@ -36,6 +36,24 @@ namespace exl3b {
 using namespace ptx;
 
 // ---- input transform into the tiled activation layout ---------------------------------------------------------
+// Tile of one unit: [NT / 8 row groups][16 K-chunks][8 rows][8 fp16], K-chunks 128 B apart, row groups 2048 B apart.  K order:
+// k = 16 kt + 4 j + 2 h + e (kt = 4 r + c) sits in K-chunk 2 (4 r + j) + h at element 2 c + e, i.e. lane l's four values
+// k = 4 l .. 4 l + 3 go to K-chunks 8 (l / 16) + 2 (l % 4) (+1 for the second pair), element pair (l / 4) % 4.
+__device__ __forceinline__ int xt_tile_offset(int r, int lane)
+{
+    return (((r >> 3) * 16 + 8 * (lane >> 4) + 2 * (lane & 3)) * 8 + (r & 7)) * 16 + 4 * ((lane >> 2) & 3);
+}
+// the two 4-byte halves land 128 B apart (consecutive K-chunks)
+__device__ __forceinline__ uint2 pack_tile_pair(half2 a, half2 b)
+{
+    uint2 o; o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
+    return o;
+}
+__device__ __forceinline__ void store_tile_pair(uint8_t* p, uint2 o)
+{
+    *reinterpret_cast<uint32_t*>(p) = o.x;
+    *reinterpret_cast<uint32_t*>(p + 128) = o.y;
+}
 template <bool HAD>
 __global__ void __launch_bounds__(128)
 had_tiled_kernel(const half* __restrict__ A, uint8_t* __restrict__ out, const half* __restrict__ suh,
@@ -59,39 +77,53 @@ had_tiled_kernel(const half* __restrict__ A, uint8_t* __restrict__ out, const ha
         a = __floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE);
         b = __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE);
     }
-    uint2 o; o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
-    const size_t off = (size_t) kb * NT * 256 + ((((r >> 3) * 16 + (lane >> 1)) * 8 + (r & 7)) * 16) + (lane & 1) * 8;
-    *reinterpret_cast<uint2*>(out + off) = o;
+    store_tile_pair(out + (size_t) kb * NT * 256 + xt_tile_offset(r, lane), pack_tile_pair(a, b));
 }
 
 // ---- the kernel -------------------------------------------------------------------------------------------------
+constexpr int XT_THREADS = 384;
+constexpr int XT_MAX_ROWS = 128;                 // activation rows per pass: NT / 16 accumulator chunks of 8 registers
+constexpr int XT_CONS_WARP0 = 4, XT_CONS_WARPS = 8;
+
+// smem: weight ring, activation ring, fp32 segment tile [NT][128], barriers
+__host__ __device__ inline TcSmemLayout xt_smem_layout(int K, int b_bytes, int stages, int NT)
+{
+    TcSmemLayout L;
+    L.w_bytes = 2048 * K;
+    L.b_bytes = b_bytes;
+    L.off_b = stages * L.w_bytes;
+    L.off_tile = L.off_b + stages * L.b_bytes;
+    L.off_bars = L.off_tile + NT * 128 * 4;
+    L.total = L.off_bars + 1024;
+    L.off_d = L.total;
+    return L;
+}
+
+// D[64 x 16] (f32) += A[64 x 16] (f16, registers) * B[16 x 16] (f16, shared memory, K-major)
+__device__ __forceinline__ void wgmma_f16_n16(float (&d)[8], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc)
+{
+    asm volatile("wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, 1, 1, 1, 0;"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc) : "memory");
+}
+
 template <int K, int cb>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__(XT_THREADS, 1)
 gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
 {
     extern __shared__ __align__(1024) uint8_t smem[];
-    const TcSmemLayout L = tc_smem_layout(K, p.b_bytes, p.stages);
+    const TcSmemLayout L = xt_smem_layout(K, p.b_bytes, p.stages, p.NT);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int S = p.stages;
 
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
-    // barrier map: [0,S) w_full  [S,2S) w_empty  [2S,3S) x_full  then a_full[4] a_empty[4] d_full[2] d_empty[2]
+    // barrier map: [0,S) w_full  [S,2S) w_empty  [2S,3S) x_full
     const uint32_t bar0 = smem_u32(bars);
     auto W_FULL = [&](int s) { return bar0 + 8u * s; };
     auto W_EMPTY = [&](int s) { return bar0 + 8u * (S + s); };
     auto X_FULL = [&](int s) { return bar0 + 8u * (2 * S + s); };
-    auto A_FULL = [&](int s) { return bar0 + 8u * (3 * S + s); };
-    auto A_EMPTY = [&](int s) { return bar0 + 8u * (3 * S + 8 + s); };
-    auto D_FULL = [&](int s) { return bar0 + 8u * (3 * S + 16 + s); };
-    auto D_EMPTY = [&](int s) { return bar0 + 8u * (3 * S + 18 + s); };
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L.off_bars + 8 * (3 * TC_MAX_STAGES + 20));
-    int* s_flag = reinterpret_cast<int*>(tmem_slot + 1);
+    int* s_flag = reinterpret_cast<int*>(smem + L.off_bars + 8 * (3 * TC_MAX_STAGES + 20));
 
-#ifdef EXL3B_TC_DEBUG
-    const int KNOB = p.knob_;
-#else
-    constexpr int KNOB = 0;
-#endif
     auto stamp = [&](int slot)
     {
 #ifdef EXL3B_TC_DEBUG
@@ -105,20 +137,11 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
 
     if (warp == 0)
     {
-        // one barrier per lane and round instead of ~70 serial initialisations by one thread
-        for (int s = lane; s < S; s += 32) { mbar_init(W_FULL(s), 1); mbar_init(X_FULL(s), 1); mbar_init(W_EMPTY(s), TC_DEC_WARPS / TC_DEC_GROUPS + 1); }
-        if (lane < 8) { mbar_init(A_FULL(lane), TC_DEC_WARPS / TC_DEC_GROUPS); mbar_init(A_EMPTY(lane), 1); }
-        else if (lane < 10) { mbar_init(D_FULL(lane - 8), 1); mbar_init(D_EMPTY(lane - 8), 4); }
+        // W_EMPTY: the eight consumer warps, after their MMAs have read the stage
+        for (int s = lane; s < S; s += 32) { mbar_init(W_FULL(s), 1); mbar_init(X_FULL(s), 1); mbar_init(W_EMPTY(s), XT_CONS_WARPS); }
         fence_barrier_init();
     }
-    if (warp == 1)
-    {
-        if (p.tmem_cols == 256) tmem_alloc<256>(smem_u32(tmem_slot)); else tmem_alloc<512>(smem_u32(tmem_slot));
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (threadIdx.x == 0) stamp(1);
 
     // ---- this CTA's unit range ----
@@ -128,125 +151,56 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
     const int G = gridDim.x;
     const long long ubeg = unit_begin(U, G, blockIdx.x), uend = unit_begin(U, G, blockIdx.x + 1);
     const int n_units = (int) (uend - ubeg);
-    const int tiles_n = p.n / 16;
-    const int a_cols0 = 0;
-    const int d_cols0 = p.a_stages * TC_A_STAGE_COLS;
 
     if (warp == 0)
     {
         // =========================== producer ===========================
         // whole warp runs the loop (uniform control flow -> uniform-register operands); one elected lane issues
+        if (elect_one()) prefetch_tmap(&tmap_w);
+        const uint64_t pol_w = policy_evict_first(), pol_x = policy_evict_last();
+        const uint32_t w_smem0 = smem_u32(smem), x_smem0 = smem_u32(smem + L.off_b);
+        auto issue_w = [&](int s, int strip, int kb)
         {
-            if (elect_one()) prefetch_tmap(&tmap_w);
-            const uint64_t pol_w = policy_evict_first(), pol_x = policy_evict_last();
-            const uint32_t w_smem0 = smem_u32(smem), x_smem0 = smem_u32(smem + L.off_b);
-            auto issue_w = [&](int s, int strip, int kb)
+            if (elect_one())
             {
-                if (elect_one())
-                {
-                    mbar_arrive_expect_tx(W_FULL(s), (uint32_t) L.w_bytes);
-                    // one 2-D TMA box per unit: 8 tile-rows x (256*K bytes = 32*K uint64) of the trellis
-                    if (KNOB & 16) tma_load_2d(w_smem0 + s * L.w_bytes, &tmap_w, 0, (strip * KB + kb) * 8, W_FULL(s), pol_w);
-                    else tma_load_2d(w_smem0 + s * L.w_bytes, &tmap_w, strip * (32 * K), kb * 8, W_FULL(s), pol_w);
-                }
-            };
-            auto issue_x = [&](int s, int kb)
-            {
-                if (elect_one())
-                {
-                    mbar_arrive_expect_tx(X_FULL(s), (uint32_t) p.b_load_bytes);
-                    bulk_g2s(x_smem0 + s * L.b_bytes, p.xh_tiled + (size_t) kb * p.NT * 256,
-                             (uint32_t) p.b_load_bytes, X_FULL(s), pol_x);
-                }
-            };
-            const int pre = n_units < S ? n_units : S;
-            const int strip0 = (int) (ubeg / KB), kb0 = (int) (ubeg % KB);
-            int strip = strip0, kb = kb0;
-            auto next_unit = [&] { if (++kb == KB) { kb = 0; ++strip; } };
-            for (int u = 0; u < pre; ++u) { issue_w(u, strip, kb); next_unit(); }   // weights never depend on the previous kernel
-            const bool fused_x = p.A_raw != nullptr;
-            if (!fused_x)
-            {
-                pdl_wait();                                                          // activations do
-                int kbx = kb0; for (int u = 0; u < pre; ++u) { issue_x(u, kbx); if (++kbx == KB) kbx = 0; }
+                mbar_arrive_expect_tx(W_FULL(s), (uint32_t) L.w_bytes);
+                // one 2-D TMA box per unit: 8 tile-rows x (256*K bytes = 32*K uint64) of the trellis
+                tma_load_2d(w_smem0 + s * L.w_bytes, &tmap_w, strip * (32 * K), kb * 8, W_FULL(s), pol_w);
             }
-            if (lane == 0) stamp(2);
-            int s = (pre == S) ? 0 : pre, ph = (pre == S) ? 1 : 0;                   // ring position of unit `pre`
-            for (int u = pre; u < n_units; ++u)
+        };
+        auto issue_x = [&](int s, int kb)
+        {
+            if (elect_one())
             {
-                mbar_wait<64>(W_EMPTY(s), ph ^ 1);
-                issue_w(s, strip, kb);
-                if (!fused_x) issue_x(s, kb);
-                next_unit();
-                if (++s == S) { s = 0; ph ^= 1; }
+                mbar_arrive_expect_tx(X_FULL(s), (uint32_t) p.b_load_bytes);
+                bulk_g2s(x_smem0 + s * L.b_bytes, p.xh_tiled + (size_t) kb * p.NT * 256,
+                         (uint32_t) p.b_load_bytes, X_FULL(s), pol_x);
             }
+        };
+        const int pre = n_units < S ? n_units : S;
+        const int strip0 = (int) (ubeg / KB), kb0 = (int) (ubeg % KB);
+        int strip = strip0, kb = kb0;
+        auto next_unit = [&] { if (++kb == KB) { kb = 0; ++strip; } };
+        for (int u = 0; u < pre; ++u) { issue_w(u, strip, kb); next_unit(); }   // weights never depend on the previous kernel
+        const bool fused_x = p.A_raw != nullptr;
+        if (!fused_x)
+        {
+            pdl_wait();                                                          // activations do
+            int kbx = kb0; for (int u = 0; u < pre; ++u) { issue_x(u, kbx); if (++kbx == KB) kbx = 0; }
+        }
+        if (lane == 0) stamp(2);
+        int s = (pre == S) ? 0 : pre, ph = (pre == S) ? 1 : 0;                   // ring position of unit `pre`
+        for (int u = pre; u < n_units; ++u)
+        {
+            mbar_wait<64>(W_EMPTY(s), ph ^ 1);
+            issue_w(s, strip, kb);
+            if (!fused_x) issue_x(s, kb);
+            next_unit();
+            if (++s == S) { s = 0; ph ^= 1; }
         }
         __syncwarp();
     }
-    else if (warp == 1)
-    {
-        // =========================== MMA issuer ===========================
-        // whole warp runs the loop; one elected lane issues the MMAs and their commits
-        {
-            const uint32_t idesc = idesc_f16_f32(128, p.NT);
-            const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-            const uint32_t x_smem0 = smem_u32(smem + L.off_b);
-            // descriptor template: LBO 128 B, SBO 2048 B, version 1, no swizzle; the start address goes in bits 0..13
-            const uint64_t desc_hi = smem_desc(0, 128, 2048, 0);
-            int dbuf = 0, dphase = 0, seg_left = 0;
-            uint32_t acc = 0;
-            int kb = (int) (ubeg % KB);
-            int s = 0, sph = 0, as = 0, aph = 0;
-            for (int u = 0; u < n_units; ++u)
-            {
-                if (seg_left == 0)
-                {
-                    // new segment: units up to the end of this strip or of this CTA's range
-                    const int to_strip_end = KB - kb;
-                    seg_left = (n_units - u) < to_strip_end ? (n_units - u) : to_strip_end;
-                    mbar_wait(D_EMPTY(dbuf), dphase ^ 1);
-                    acc = 0;
-                }
-                mbar_wait(X_FULL(s), sph);
-                mbar_wait(A_FULL(as), aph);
-                tc_fence_after();
-                if (u == 0 && lane == 0) stamp(5);
-                const uint32_t d_addr = tb + d_cols0 + dbuf * p.NT;
-                const uint32_t a_addr = tb + a_cols0 + as * TC_A_STAGE_COLS;
-                const uint32_t b_addr = x_smem0 + s * L.b_bytes;
-                --seg_left;
-                if (elect_one())
-                {
-                    if (!(KNOB & 4))
-                    {
-                        #pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                        {
-                            mma_f16_ts(d_addr, a_addr + 8 * j, desc_hi | (uint64_t) (((b_addr + j * 256) >> 4) & 0x3fff),
-                                       idesc, acc);
-                            acc = 1;
-                        }
-                    }
-                    tc_commit(A_EMPTY(as));
-                    tc_commit(W_EMPTY(s));
-                    if (seg_left == 0) tc_commit(D_FULL(dbuf));
-                }
-                acc = 1;
-                __syncwarp();
-                if (seg_left == 0)
-                {
-                    if (p.d_bufs == 2) { dbuf ^= 1; if (dbuf == 0) dphase ^= 1; }
-                    else dphase ^= 1;
-                }
-                if (++kb == KB) kb = 0;
-                if (++s == S) { s = 0; sph ^= 1; }
-                if (++as == p.a_stages) { as = 0; aph ^= 1; }
-            }
-            if (lane == 0) stamp(6);
-        }
-        __syncwarp();
-    }
-    else if (warp < TC_DEC_WARP0)
+    else if (warp >= TC_XF_WARP0 && warp < XT_CONS_WARP0)
     {
         // =========================== fused input transform (m <= 8) ===========================
         if (p.A_raw != nullptr)
@@ -275,8 +229,7 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
                         a = __floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE);
                         b = __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE);
                     }
-                    uint2 o; o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
-                    *reinterpret_cast<uint2*>(dst + ((((r >> 3) * 16 + (lane >> 1)) * 8 + (r & 7)) * 16) + (lane & 1) * 8) = o;
+                    store_tile_pair(dst + xt_tile_offset(r, lane), pack_tile_pair(a, b));
                 }
                 fence_proxy_async_smem();                // generic-proxy writes -> visible to the tensor-core (async) proxy
                 __syncwarp();
@@ -286,79 +239,38 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
             }
         }
     }
-    else if (warp >= TC_DEC_WARP0 && warp < TC_DEC_WARP0 + TC_DEC_WARPS)
+    else if (warp >= XT_CONS_WARP0)
     {
-        // =========================== decode ===========================
-        // Four groups of four warps (one warp per TMEM lane quarter); group g owns the units u = g (mod 4) and decodes
-        // ALL eight k-tiles of them, so the per-unit handshake cost (two mbarrier waits, shuffles, tcgen05.wait::st,
-        // two arrives: ~300 ns measured) is paid once per 8 tiles per warp and the groups run out of lockstep.
-        const int q = warp & 3, g = (warp - TC_DEC_WARP0) >> 2;
-        const int tl = strip_tile(q, lane), chunk = lane & 7;
-        const int prev_lane = (lane & ~7) | ((lane + 7) & 7);
-        const uint32_t lane_base = (uint32_t) (q * 32) << 16;
-        int s = g % S, sph = (g / S) & 1, as = g % p.a_stages, aph = (g / p.a_stages) & 1;
-        const int s_step = TC_DEC_GROUPS % S, s_wrap = TC_DEC_GROUPS / S;                       // ring stride of a group
-        const int a_step = TC_DEC_GROUPS % p.a_stages, a_wrap = TC_DEC_GROUPS / p.a_stages;
-        for (int u = g; u < n_units; u += TC_DEC_GROUPS)
-        {
-            mbar_wait<32>(W_FULL(s), sph);
-            if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) stamp(3);
-            const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
-            #pragma unroll
-            for (int half = 0; half < 2; ++half)
-            {
-                uint32_t w[4][K + 1];
-                tc_load_tiles4<K>(wst, tl, chunk, prev_lane, half * 4, 1, w);
-                if (half == 0) { mbar_wait(A_EMPTY(as), aph ^ 1); tc_fence_after(); }
-                #pragma unroll
-                for (int j = 0; j < 4; ++j)
-                {
-                    const int t = half * 4 + j;
-                    uint32_t o[8];
-                    if (KNOB & 1)
-                    {
-                        #pragma unroll
-                        for (int i = 0; i < 8; ++i) o[i] = w[j][i % (K + 1)];
-                    }
-                    else if (q & 1) decode16<K, cb, 1>(w[j], o); else decode16<K, cb, 0>(w[j], o);
-                    if (!(KNOB & 2))
-                        tmem_st_32x32b_x8(tmem_base + lane_base + a_cols0 + as * TC_A_STAGE_COLS + 8 * t, o);
-                    else if (o[0] == 0x12345678u && o[7] == 0x9abcdef0u) p.counters[0] = 1;     // keep the values alive
-                }
-            }
-            tc_wait_st();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(A_FULL(as)); mbar_arrive(W_EMPTY(s)); }
-            if (warp == TC_DEC_WARP0 && lane == 0 && u == 0) stamp(4);
-            if (q == 0 && lane == 0 && u == n_units - 1) stamp(10);
-            { const int t = s + s_step; const int c = t >= S; s = c ? t - S : t; sph ^= (s_wrap + c) & 1; }
-            { const int t = as + a_step; const int c = t >= p.a_stages; as = c ? t - p.a_stages : t; aph ^= (a_wrap + c) & 1; }
-        }
-    }
-    else if (warp >= TC_EPI_WARP0)
-    {
-        // =========================== epilogue ===========================
-        pdl_wait();                                   // no global write before the previous grid has fully completed
-        const int q = warp & 3;
-        const int et = threadIdx.x - TC_EPI_WARP0 * 32;          // 0..127
-        const int col = strip_col(q, lane);
-        const uint32_t lane_base = (uint32_t) (q * 32) << 16;
-        float* tile = reinterpret_cast<float*>(smem + L.off_tile);
-        auto epi_bar = [] { asm volatile("bar.sync 1, 128;" ::: "memory"); };
+        // =========================== decode + MMA + epilogue (two warpgroups) ===========================
+        const int ct = threadIdx.x - XT_CONS_WARP0 * 32;             // 0..255
+        const int cw = ct >> 5;                                      // consumer warp 0..7
+        const int h = cw >> 2, wq = cw & 3;
+        const int tl = 4 * h + wq;                                   // tile column of the strip owned by this warp
+        const int chunk = lane >> 2, c = lane & 3;
+        const int nchunks = p.NT / 16;
+        float* tile = reinterpret_cast<float*>(smem + L.off_tile);   // [NT][128] fp32: one strip's k-segment sums
+        auto cons_bar = [] { asm volatile("bar.sync 1, 256;" ::: "memory"); };
         const int part_stride = p.NT * 128;
+        const uint64_t desc0 = smem_desc(smem_u32(smem + L.off_b), 128, 2048, 0);
+        pdl_wait();                                                  // no global write before the previous grid has completed
 
-        // rows [c0, c0+16) of one strip: tile (fp32 sums) -> output transform -> C
-        auto emit_rows = [&](int strip, int c0)
+        float acc[XT_MAX_ROWS / 16][8];
+        #pragma unroll
+        for (int i = 0; i < XT_MAX_ROWS / 16; ++i)
+            #pragma unroll
+            for (int e = 0; e < 8; ++e) acc[i][e] = 0.f;
+
+        // all rows of one strip: tile (fp32 sums) -> output transform -> C
+        auto emit_rows = [&](int strip)
         {
-            epi_bar();
-            for (int j = q; j < 16 && c0 + j < p.m; j += 4)
-                output_row_128(tile + j * 128, (char*) p.C, (size_t) (c0 + j) * p.n + strip * 128,
+            cons_bar();
+            for (int j = cw; j < p.m; j += XT_CONS_WARPS)
+                output_row_128(tile + j * 128, (char*) p.C, (size_t) j * p.n + strip * 128,
                                p.svh ? p.svh + strip * 128 : nullptr, p.out_scale, p.c_fp32 != 0, lane);
-            epi_bar();
+            cons_bar();
         };
 
-        int dbuf = 0, dphase = 0;
+        int s = 0, sph = 0;
         int u = 0;
         while (u < n_units)
         {
@@ -372,38 +284,80 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
             const bool full = n_contrib == 1;
             float* my_part = p.ws + (size_t) (2 * blockIdx.x + (ubeg >= gs ? 0 : 1)) * part_stride;
 
-            mbar_wait<32>(D_FULL(dbuf), dphase);
-            tc_fence_after();
-            if (u == 0 && et == 0) stamp(7);
-            const uint32_t d_addr = tmem_base + lane_base + d_cols0 + dbuf * p.NT;
-            for (int c0 = 0; c0 < p.m; c0 += 16)
+            for (int i = 0; i < seg; ++i)
             {
-                uint32_t r[16];
-                tmem_ld_32x32b_x16(d_addr + c0, r);
-                tc_wait_ld();
-                if (full)
+                mbar_wait<32>(W_FULL(s), sph);
+                if (u + i == 0 && ct == 0) stamp(3);
+                const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
+                uint32_t w[2][K + 1];
+                #pragma unroll
+                for (int r = 0; r < 2; ++r) load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, w[r]);
+                mbar_wait(X_FULL(s), sph);
+                const uint64_t desc_s = desc0 + (uint64_t) ((s * L.b_bytes) >> 4);
+                #pragma unroll
+                for (int r = 0; r < 2; ++r)
                 {
+                    uint32_t o0[8], o1[8];
+                    decode16<K, cb, 0>(w[r], o0);
+                    decode16<K, cb, 1>(w[r], o1);
                     #pragma unroll
-                    for (int j = 0; j < 16; ++j) tile[j * 128 + col] = __uint_as_float(r[j]);
-                    emit_rows(strip, c0);
-                }
-                else
-                {
+                    for (int ii = 0; ii < XT_MAX_ROWS / 16; ++ii)
+                        #pragma unroll
+                        for (int e = 0; e < 8; ++e) reg_fence(acc[ii][e]);
+                    wgmma_fence();
                     #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (c0 + j < p.m) my_part[(c0 + j) * 128 + col] = __uint_as_float(r[j]);
+                    for (int j = 0; j < 4; ++j)
+                    {
+                        // instruction 4 r + j: K-chunks 2 (4 r + j), +1;  N-chunk ii: row groups 2 ii, 2 ii + 1
+                        #pragma unroll
+                        for (int ii = 0; ii < XT_MAX_ROWS / 16; ++ii)
+                            if (ii < nchunks)
+                                wgmma_f16_n16(acc[ii], o0[2 * j], o1[2 * j], o0[2 * j + 1], o1[2 * j + 1],
+                                              desc_s + (uint64_t) (16 * (4 * r + j) + 256 * ii));
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    #pragma unroll
+                    for (int e = 0; e < 8; ++e) { reg_fence(o0[e]); reg_fence(o1[e]); }
+                    #pragma unroll
+                    for (int ii = 0; ii < XT_MAX_ROWS / 16; ++ii)
+                        #pragma unroll
+                        for (int e = 0; e < 8; ++e) reg_fence(acc[ii][e]);
                 }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(W_EMPTY(s));
+                if (++s == S) { s = 0; sph ^= 1; }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(D_EMPTY(dbuf));
-            if (p.d_bufs == 2) { dbuf ^= 1; if (dbuf == 0) dphase ^= 1; }
-            else dphase ^= 1;
 
-            if (!full)
+            // accumulators -> tile[row][column]: fragment (row 16 ii + 2 c + e (+8), column 16 tl + chunk (+8))
+            cons_bar();                                              // the previous segment's readers of the tile are done
+            const int n0 = 16 * tl + chunk;
+            #pragma unroll
+            for (int ii = 0; ii < XT_MAX_ROWS / 16; ++ii)
             {
-                epi_bar();                                    // all partial stores of this CTA are ordered before ...
-                if (et == 0)
+                if (ii < nchunks)
+                {
+                    const int r0 = 16 * ii + 2 * c;
+                    tile[(r0 + 0) * 128 + n0] = acc[ii][0];
+                    tile[(r0 + 1) * 128 + n0] = acc[ii][1];
+                    tile[(r0 + 0) * 128 + n0 + 8] = acc[ii][2];
+                    tile[(r0 + 1) * 128 + n0 + 8] = acc[ii][3];
+                    tile[(r0 + 8) * 128 + n0] = acc[ii][4];
+                    tile[(r0 + 9) * 128 + n0] = acc[ii][5];
+                    tile[(r0 + 8) * 128 + n0 + 8] = acc[ii][6];
+                    tile[(r0 + 9) * 128 + n0 + 8] = acc[ii][7];
+                }
+                #pragma unroll
+                for (int e = 0; e < 8; ++e) acc[ii][e] = 0.f;
+            }
+            if (u + seg >= n_units && ct == 0) stamp(7);
+            if (full) emit_rows(strip);
+            else
+            {
+                cons_bar();
+                for (int idx = ct; idx < p.m * 128; idx += 256) my_part[idx] = tile[idx];
+                cons_bar();                                   // all partial stores of this CTA are ordered before ...
+                if (ct == 0)
                 {
                     __threadfence();                          // ... this single gpu-scope fence + the arrival count (cumulativity)
                     const int old = atomicAdd(&p.counters[strip], 1);
@@ -411,45 +365,28 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
                     if (last) { p.counters[strip] = 0; __threadfence(); }          // self-reset for the next launch using this slot
                     *s_flag = last;
                 }
-                epi_bar();
+                cons_bar();
                 if (*s_flag)
                 {
                     const int which_a = unit_begin(U, G, c_a) >= gs ? 0 : 1;       // only c_a can have started in an earlier strip
-                    for (int c0 = 0; c0 < p.m; c0 += 16)
+                    for (int idx = ct; idx < p.m * 128; idx += 256)
                     {
-                        float acc[16];
-                        #pragma unroll
-                        for (int j = 0; j < 16; ++j) acc[j] = 0.f;
-                        for (int c = c_a; c <= c_b; ++c)                 // fixed order: deterministic
-                        {
-                            const float* part = p.ws + (size_t) (2 * c + (c == c_a ? which_a : 0)) * part_stride;
-                            float v[16];
-                            #pragma unroll
-                            for (int j = 0; j < 16; ++j) v[j] = (c0 + j < p.m) ? __ldcg(part + (c0 + j) * 128 + col) : 0.f;
-                            #pragma unroll
-                            for (int j = 0; j < 16; ++j) acc[j] += v[j];
-                        }
-                        #pragma unroll
-                        for (int j = 0; j < 16; ++j) tile[j * 128 + col] = acc[j];
-                        emit_rows(strip, c0);
+                        float a = 0.f;
+                        for (int cc = c_a; cc <= c_b; ++cc)                        // fixed order: deterministic
+                            a += __ldcg(p.ws + (size_t) (2 * cc + (cc == c_a ? which_a : 0)) * part_stride + idx);
+                        tile[idx] = a;
                     }
+                    emit_rows(strip);
                 }
-                epi_bar();
             }
             u += seg;
         }
-        if (et == 0) stamp(8);
+        if (ct == 0) stamp(8);
     }
 
     // ---- teardown ----
-    tc_fence_before();
     __syncthreads();
     if (threadIdx.x == 0) stamp(9);
-    if (warp == 1)
-    {
-        tc_fence_after();
-        if (p.tmem_cols == 256) tmem_dealloc<256>(tmem_base); else tmem_dealloc<512>(tmem_base);
-    }
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------
@@ -515,7 +452,7 @@ static cudaError_t tc_launch(cudaStream_t stream, int grid, int smem_bytes, cons
         attr_set[dev & 31] = true;
     }
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(XT_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
@@ -563,12 +500,9 @@ static int launch_had_tiled(cudaStream_t stream, const half* A, uint8_t* out, co
     return 0;
 }
 
-// In-kernel input transform (two warps, per unit) or the separate had_tiled launch + tile loads?  Measured (round 2,
-// profiles/r02_notes.md 5; us per call, in-kernel vs tiled): 5 rows 16.0 vs 13.7 (4096 x 4096), 33.4 vs 22.8 (4096 x 14336),
-// 34.8 vs 24.2 (14336 x 4096); 8 rows 19.3 vs 13.7, 44.5 vs 22.9, 46.1 vs 25.9 -- the two transform warps pace the kernel from five
-// rows on (one 128-point Hadamard per row and unit).  At 1..4 rows (3INST codebook) the two are equal on 4096 x 4096 (13.5 us) and the
-// tiled path is ahead on 4096 x 14336 (24.4 vs 25.0 us at 1 row, 24.4 vs 30.3 at 4 rows), so the tiled path is the default for every
-// row count; EXL3B_FUSED_X_ROWS=r (<= 8) brings the in-kernel transform back for up to r rows.
+// In-kernel input transform (two warps, per unit) or the separate had_tiled launch + tile loads?  The two transform warps do one
+// 128-point Hadamard per row and unit and pace the kernel as rows grow, so the tiled path is the default for every row count;
+// EXL3B_FUSED_X_ROWS=r (<= 8) brings the in-kernel transform back for up to r rows.
 static bool tc_fused_x(int m, int k, int n, int num_sms)
 {
     (void) k; (void) n; (void) num_sms;
@@ -582,25 +516,24 @@ static bool tc_fused_x(int m, int k, int n, int num_sms)
     return m <= max_rows;
 }
 
-// launch geometry of one pass (m <= 256 rows), also behind exl3b_gemm_plan
+// launch geometry of one pass (m <= XT_MAX_ROWS rows), also behind exl3b_gemm_plan
 int plan_gemm_tc(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* pl)
 {
-    EXL3B_CHECK(m >= 1 && m <= 256, EXL3B_ERR_ARG, "plan_gemm_tc: one pass handles 1..256 rows");
+    EXL3B_CHECK(m >= 1 && m <= XT_MAX_ROWS, EXL3B_ERR_ARG, "plan_gemm_tc: one pass handles 1..%d rows", XT_MAX_ROWS);
     const int NT = (m + 15) / 16 * 16;
     const bool fused_x = tc_fused_x(m, k, n, num_sms);
-    // all of TMEM: the operand-stage loop (decode -> tcgen05.st -> MMA -> commit -> decode) has ~1.3 us of latency;
-    // the number of 64-column A stages in flight is what hides it (measured: 3 stages = 450 ns per unit floor)
-    pl->tmem_cols = 512;
-    pl->a_stages = NT <= 32 ? 7 : 4;
-    pl->d_bufs = NT <= 128 ? 2 : 1;
+    // accumulators live in the consumer warpgroups' registers: no operand stages or accumulator buffers to plan
+    pl->tmem_cols = 0;
+    pl->a_stages = 0;
+    pl->d_bufs = 1;
     pl->b_load_bytes = m <= 8 ? 2048 : NT * 256;
     const int b_bytes = fused_x ? 2048 : NT * 256;       // m <= 8: only the first row group is ever written / needed
     const int stage_bytes = 2048 * K + b_bytes;
-    const int budget = 200 * 1024;
+    const int budget = 200 * 1024 - NT * 128 * 4;
     int stages = budget / stage_bytes;
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
     if (stages < 2) stages = 2;
-    const TcSmemLayout L = tc_smem_layout(K, b_bytes, stages);
+    const TcSmemLayout L = xt_smem_layout(K, b_bytes, stages, NT);
     EXL3B_CHECK(L.total <= 220 * 1024, EXL3B_ERR_UNSUPPORTED, "exl3_gemm: shared-memory budget exceeded");
     const long long U = (long long) (k / 128) * (n / 128);
     int grid = num_sms;
@@ -618,9 +551,9 @@ int launch_gemm_tc(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
     const size_t esz = a.c_fp32 ? 4 : 2;
     CUtensorMap tmap;
     { int r = get_weight_tmap(a.B, a.k, a.n, a.K, &tmap); if (r) return r; }
-    for (int m0 = 0; m0 < a.m; m0 += 256)
+    for (int m0 = 0; m0 < a.m; m0 += XT_MAX_ROWS)
     {
-        const int m = a.m - m0 < 256 ? a.m - m0 : 256;
+        const int m = a.m - m0 < XT_MAX_ROWS ? a.m - m0 : XT_MAX_ROWS;
         TcPlan pl;
         { int r = plan_gemm_tc(m, a.k, a.n, a.K, ctx->num_sms, a.max_ctas, &pl); if (r) return r; }
         const int NT = pl.rows;
@@ -639,9 +572,6 @@ int launch_gemm_tc(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
         p.xh_tiled = xh_tiled; p.B = a.B; p.C = (char*) a.C + (size_t) m0 * a.n * esz; p.svh = a.svh;
         p.m = m; p.k = a.k; p.n = a.n; p.NT = NT; p.c_fp32 = a.c_fp32; p.out_scale = a.out_scale;
         p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot);
-        p.tmem_cols = pl.tmem_cols;
-        p.a_stages = pl.a_stages;
-        p.d_bufs = pl.d_bufs;
         p.b_load_bytes = pl.b_load_bytes;
         p.stages = pl.stages;
         p.dbg = g_tc_dbg;

@@ -1,4 +1,4 @@
-// Plain (single-GPU / column-parallel) instantiations and host side of the tcgen05 kind::i8 EXL3 decode-GEMM;
+// Plain (single-GPU / column-parallel) instantiations and host side of the wgmma u8 x s8 EXL3 decode-GEMM;
 // the kernel itself is in gemm_tc_i8_body.cuh.
 #include "gemm_tc_i8_body.cuh"
 
@@ -55,7 +55,7 @@ int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPla
     int cache_bytes = m * k * 2;
     cache_bytes = (cache_bytes + 127) / 128 * 128;
     if (cache_bytes > I8_CACHE_MAX_BYTES) cache_bytes = 0;
-    int stages = (200 * 1024 - cache_bytes) / stage_bytes;
+    int stages = (200 * 1024 - i8_d_bytes(MR) - cache_bytes) / stage_bytes;
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
     if (stages < 2) stages = 2;
     const TcSmemLayout L = i8_smem_layout(K, MR, stages, cache_bytes);
@@ -67,7 +67,7 @@ int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPla
     EXL3B_CHECK(n / 128 <= DevCtx::COUNTERS_PER_SLOT, EXL3B_ERR_UNSUPPORTED, "exl3_gemm: too many column strips");
     EXL3B_CHECK(grid <= DevCtx::I8_PART_CTAS, EXL3B_ERR_UNSUPPORTED, "exl3_gemm (i8): grid exceeds the split-K exchange buffer");
     pl->rows = MR; pl->stages = stages; pl->b_bytes = i8_b_stage(MR); pl->b_load_bytes = cache_bytes; pl->smem_total = L.total;
-    pl->grid = grid; pl->units = U; pl->a_stages = I8_A_STAGES; pl->d_bufs = 2; pl->tmem_cols = 512;
+    pl->grid = grid; pl->units = U; pl->a_stages = 0; pl->d_bufs = 2; pl->tmem_cols = 0;
     return 0;
 }
 
@@ -173,7 +173,7 @@ int launch_mgemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a)
     int cache_bytes = a.m * a.k * 2;
     cache_bytes = (cache_bytes + 127) / 128 * 128;
     if (cache_bytes > I8_CACHE_MAX_BYTES) cache_bytes = 0;
-    int stages = (200 * 1024 - cache_bytes) / stage_bytes;
+    int stages = (200 * 1024 - i8_d_bytes(MR) - cache_bytes) / stage_bytes;
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
     if (stages < 2) stages = 2;
     p.stages = stages; p.b_bytes = i8_b_stage(MR); p.b_load_bytes = cache_bytes;

@@ -12,7 +12,7 @@
 // "peer" buffers to local allocations so that the protocol can be exercised on one GPU (tests, bring-up).
 //
 // STATUS: world-1 equality with the plain kernel and the loop-back protocol (scatter, rank-ordered sum, re-arming, slot
-// alternation) verified on a B200 in round 2; multi-GPU runs: tests/test_tp_fused.py -m multigpu, bench.py --gpus N.
+// alternation) tested on one GPU; multi-GPU runs: tests/test_tp_fused.py -m multigpu, bench.py --gpus N.
 #include "gemm_tc_i8_body.cuh"
 #include <mutex>
 
@@ -89,7 +89,7 @@ int tp_alloc(int rank, int world, long long max_elems, void* handle_out)
                 "tp_alloc: max_elems (%lld) must be a multiple of 128 in [128, 2^26]", max_elems);
     { int r = tp_free(); if (r) return r; }
     TpGroup* g; int r = tp_current(&g); if (r) return r;
-    DevCtx* ctx; r = get_ctx(&ctx); if (r) return r;                 // also rejects non-sm_100 devices
+    DevCtx* ctx; r = get_ctx(&ctx); if (r) return r;                 // also rejects devices other than sm_90
     std::lock_guard<std::mutex> lock(g_tp_mutex);
     g->rank = rank; g->world = world; g->slot_elems = max_elems;
     EXL3B_CUDA(cudaMalloc(&g->local, tp_buffer_bytes(*g)));

@@ -1,15 +1,14 @@
-// tcgen05 kind::i8 EXL3 decode-GEMM for the mul1 codebook, m <= 4 (instantiated for up to 8 rows, see api.cu) ("TC-i8 path", tag 210).
+// wgmma u8 x s8 EXL3 decode-GEMM for the mul1 codebook, m <= 4 (instantiated for up to 8 rows, see api.cu) ("TC-i8 path", tag 210).
 //
-// Why: the bit-exact mul1 decode needs IMAD + IDP.4A per weight on the same issue pipe plus pack + HFMA2; measured
-// (profiles/r01_microbench_pipes.log) that caps the decode at ~20 weights/clk/SM = ~45 % of the HBM rate at K = 4.
+// Why: the bit-exact mul1 decode needs IMAD + IDP.4A per weight on the same issue pipe plus pack + HFMA2.
 // The mul1 value is AFFINE in the byte sum of x = state * 0x83DCD12D:
 //        w = k_inv * (1024 + b0 + b1 + b2 + b3) + k_bias              (codebook.cuh:77-89, before its fp16 rounding)
 // so   sum_k a_k w_kn = k_inv * sum_k a_k (b0+b1+b2+b3)_kn + (1024 k_inv + k_bias) * sum_k a_k.
 // The first sum is an integer GEMM whose K-elements are the four product BYTES: the decode thread stores the raw
-// 32-bit product into a TMEM kind::i8 A operand (4 u8 along K) and the tensor core sums the bytes while contracting
+// 32-bit product into a register A operand of wgmma (4 u8 along K) and the tensor core sums the bytes while contracting
 // with the activation, which is quantised per row to a balanced pair of signed 8-bit digits (q = 256 hi + lo,
 // |q| <= 32512, i.e. 16-bit activations; hi and lo are two N-columns, each digit replicated over the 4 bytes).
-// Per weight that leaves window extraction + ONE IMAD (measured mix: 42.7 weights/clk/SM).
+// Per weight that leaves window extraction + ONE IMAD.
 //
 // Numerics: integer accumulation is exact; what differs from the reference's fp16 kernel is (a) the per-weight fp16
 // rounding of the codebook value is skipped (rel-RMS ~3e-4 of the output, unbiased) and (b) activations carry
@@ -17,20 +16,20 @@
 // its int8-activation GEMV with ~0.9 % output RMS deviation (exl3_gemv_int8.cu:19-20); this path is ~30x closer to
 // the fp16 kernel than that.  Tolerances are asserted in tests/test_gpu_parity.py::test_gemm_i8_*.
 //
-// Structure is the same as gemm_tc.cu (stream-K units of 128x128 weights, TMA ring, TMEM operand stages, warp roles);
-// differences:
-//   * A stage = 128 TMEM columns (one 32-bit product per weight, three stages), 16 MMAs (K = 32 bytes = 8 weights) per unit
-//     issued from one stepped shared-memory descriptor (one uniform add per MMA), int32 accumulators
+// Structure: stream-K units of 128x128 weights, a TMA ring of weight stages, warp roles:
+//   * four decode warpgroups (warps 4..19): warpgroup (g, nh) takes the units u = g (mod 2) and their 64 output columns
+//     nh*64 .. nh*64+63.  A warp owns one 16x16-tile column of the strip; lane (chunk, c) decodes tile column `chunk`, both
+//     halves, of k-tile 4r + c (r = 0, 1).  Its 2 x 16 products ARE the wgmma A fragments (rows chunk / chunk + 8, K slots
+//     c / c + 4) of 8 wgmma.m64nNk32 per r; the K order inside each instruction is permuted accordingly in the digit tile.
+//     int32 accumulators stay in registers for a sub-segment and are then handed to the epilogue through shared memory
 //   * a CTA prologue (warps 2..19, redundantly per CTA) transforms the rows once into a shared-memory cache and finds the
 //     per-row |xh| maximum; the two transform warps then write per-unit activation digits + digit sums
-//   * the decode group's lead warp waits for the digits before it arrives on A_FULL, so the MMA warp polls one barrier per unit
 //   * split-K partial sums travel through a sentinel-armed exchange buffer: contributors store and leave, the CTA owning the
 //     strip's first k-segment (it processes it last) adds them to its registers in fixed CTA order and re-arms the slots --
 //     no fence, no ticket, one global round trip, bit-reproducible
 //   * multi-matrix launches (dense exl3_mgemm: the model's k+v and gate+up calls): the grid is cut into one CTA group per
 //     matrix; the pointer tables stay in device memory, each CTA patches the weight tensor map's address on the device
 //   * instantiated for MR = 4 and MR = 8 activation rows (digit tile with one / two row groups); api.cu auto-selects m <= 4
-// Measured history and the experiments that were not kept: profiles/r01_ncu_notes.md.
 #pragma once
 #include "tc_common.cuh"
 #include "i8_math.cuh"
@@ -39,39 +38,13 @@ namespace exl3b {
 
 using namespace ptx;
 
-// Experiment switch (round 2, to be timed on hardware): K = 4 decode without the per-tile half branch (decode16_i8_k4_rt).
-// Arithmetic verified on the host (tests/test_decode_emu.py).  Static effect on gemm_tc_i8_kernel<4, 4> (cuobjdump, 12.9):
-// the decode loop body shrinks from ~370 to ~320 SASS lines (one SHF more per four weights on the half-1 warps, the
-// per-tile branch / reconvergence instructions gone), but ptxas then overlaps the four tiles of a unit (64 product
-// registers live), goes from 72 to 80 registers and spills ~10 loop-carried words per unit -- whether that is a net win is
-// a measurement, not a guess.  Off: the shipped kernels are unchanged (SASS identical).
-#ifndef EXL3B_I8_K4_BRANCHFREE
-#define EXL3B_I8_K4_BRANCHFREE 0
-#endif
-
-// Round-2 experiments on the unit pipeline (each a second build of the library, timed in the same run; profiles/r02_notes.md):
-//   EXL3B_I8_PREFETCH    the decode warps load the NEXT unit's weight words (LDS + shuffles) right after the last decode of the
-//                        current one, i.e. during tcgen05.wait::st, if that ring stage has already landed (non-blocking probe)
-//   EXL3B_I8_HALF_STAGE  an operand stage is released in two halves (after the 8th and the 16th MMA of its unit): the next writer's
-//                        first tiles start ~180 cycles earlier
-#ifndef EXL3B_I8_PREFETCH
-#define EXL3B_I8_PREFETCH 0
-#endif
-#ifndef EXL3B_I8_HALF_STAGE
-#define EXL3B_I8_HALF_STAGE 0
-#endif
-#ifndef EXL3B_I8_ROWCOPY
-#define EXL3B_I8_ROWCOPY 0
-#endif
-
 constexpr int I8_MAX_M = 8;                                    // rows per launch: kernel instantiated for MR = 4 and MR = 8 rows
-constexpr int I8_A_STAGE_COLS = 128;
-constexpr int I8_A_STAGES = 3;
 constexpr int I8_DEC_GROUPS = 2;
-constexpr int I8_D_COL0 = I8_A_STAGES * I8_A_STAGE_COLS;      // 384
 constexpr int I8_NT = 16;                                      // N: rows 2r = hi digit, 2r+1 = lo digit of row r
 // digit tile of a unit: 32 K-chunks x (8 N-rows x 16 B) per row group; N-rows 2r / 2r+1 = hi / lo digit of activation row r, so
-// MR = 4 rows fill one row group (4096 B) and MR = 8 rows two (SBO = 4096 B); + 64 B of per-row digit sums behind the tile
+// MR = 4 rows fill one row group (4096 B) and MR = 8 rows two (SBO = 4096 B); + 64 B of per-row digit sums behind the tile.
+// K order: the value of unit k-index 16 kt + 2 j + b (kt = 4 r + c) sits in K-chunk 2 (8 r + j) + b at byte 4 c -- the slot the
+// decode lane holding that weight feeds to wgmma (8 r + j).
 __host__ __device__ constexpr int i8_b_bytes(int MR) { return MR <= 4 ? 4096 : 8192; }
 __host__ __device__ constexpr int i8_b_stage(int MR) { return i8_b_bytes(MR) + 64; }
 constexpr int I8_SUB_UNITS = 96;                               // int32 accumulator safety: <= 12288 k per accumulation
@@ -79,13 +52,18 @@ constexpr uint32_t I8_SENTINEL = 0xffffffffu;                  // "no partial su
 
 // optional shared-memory cache of the whole transformed activation (m x k fp16) and of the per-block digit sums, filled by
 // the CTA prologue: the per-unit transform then is an 8-byte LDS + quantise instead of a global load + Hadamard
-// (measured: the two transform warps were the per-unit critical path, ~900 cycles of latency per unit each)
+// (without it the two transform warps do a global load and a Hadamard per row and unit, on the per-unit critical path)
 constexpr int I8_CACHE_MAX_BYTES = 64 * 1024;
+
+// accumulator hand-off to the epilogue: [2 buffers][2 decode groups][128 columns][2 MR] int32, then [2][2][8] digit sums
+__host__ __device__ constexpr int i8_d_bytes(int MR) { return 2 * 2 * 128 * 2 * MR * 4 + 2 * 2 * 8 * 4; }
 
 __host__ __device__ inline TcSmemLayout i8_smem_layout(int K, int MR, int stages, int cache_bytes)
 {
     TcSmemLayout L = tc_smem_layout(K, i8_b_stage(MR), stages);
-    L.total += cache_bytes;            // cache lives after the barrier block, at the old L.total
+    L.off_d = L.total;                 // accumulator hand-off after the barrier block
+    L.total += i8_d_bytes(MR);
+    L.total += cache_bytes;            // cache after that
     return L;
 }
 
@@ -101,6 +79,8 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     extern __shared__ __align__(1024) uint8_t smem[];
     constexpr int I8_B_BYTES = i8_b_bytes(MR);
     const TcSmemLayout L = i8_smem_layout(K, MR, p.stages, 0);          // offsets only; the cache starts at L.total
+    int32_t* const s_d = reinterpret_cast<int32_t*>(smem + L.off_d);     // accumulator hand-off, [dbuf][group][128][2 MR]
+    int* const s_dt = reinterpret_cast<int*>(smem + L.off_d + i8_d_bytes(MR) - 2 * 2 * 8 * 4);   // digit sums, [dbuf][group][8]
     const bool cached = p.b_load_bytes > 0;                            // host: cache_bytes (0 = recompute per unit)
     half* xh_cache = reinterpret_cast<half*>(smem + L.total);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -150,15 +130,11 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     auto W_FULL = [&](int s) { return bar0 + 8u * s; };
     auto W_EMPTY = [&](int s) { return bar0 + 8u * (S + s); };
     auto X_FULL = [&](int s) { return bar0 + 8u * (2 * S + s); };
-    auto A_FULL = [&](int s) { return bar0 + 8u * (3 * S + s); };
-    auto A_EMPTY = [&](int s) { return bar0 + 8u * (3 * S + 4 + s); };
     auto D_FULL = [&](int s) { return bar0 + 8u * (3 * S + 8 + s); };
     auto D_EMPTY = [&](int s) { return bar0 + 8u * (3 * S + 10 + s); };
-    [[maybe_unused]] auto A_EMPTY_HI = [&](int s) { return bar0 + 8u * (3 * S + 12 + s); };      // second half of an operand stage (EXL3B_I8_HALF_STAGE)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L.off_bars + 8 * (3 * TC_MAX_STAGES + 16));
-    unsigned int* s_absmax = reinterpret_cast<unsigned int*>(tmem_slot + 4);      // [MR] float bits, >= 0
-    int* s_tout = reinterpret_cast<int*>(tmem_slot + 12);                           // [2][MR] digit sums per D buffer
-    [[maybe_unused]] volatile unsigned int* s_ar = reinterpret_cast<volatile unsigned int*>(tmem_slot + 28);   // AR: epoch of this launch
+    uint32_t* misc = reinterpret_cast<uint32_t*>(smem + L.off_bars + 8 * (3 * TC_MAX_STAGES + 16));
+    unsigned int* s_absmax = reinterpret_cast<unsigned int*>(misc + 4);           // [MR] float bits, >= 0
+    [[maybe_unused]] volatile unsigned int* s_ar = reinterpret_cast<volatile unsigned int*>(misc + 28);   // AR: epoch of this launch
 
 #ifdef EXL3B_TC_DEBUG
     const int KNOB = p.knob_;
@@ -185,18 +161,14 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
 
     if (warp == 0)
     {
-        // one barrier per lane and round instead of ~60 serial initialisations by one thread (0.3 us of every launch)
-        for (int s = lane; s < S; s += 32) { mbar_init(W_FULL(s), 1); mbar_init(X_FULL(s), 1); mbar_init(W_EMPTY(s), TC_DEC_WARPS / I8_DEC_GROUPS + 1); }
-        if (lane < 4) { mbar_init(A_FULL(lane), TC_DEC_WARPS / I8_DEC_GROUPS); mbar_init(A_EMPTY(lane), 1); mbar_init(A_EMPTY_HI(lane), 1); }
-        else if (lane < 6) { mbar_init(D_FULL(lane - 4), 1); mbar_init(D_EMPTY(lane - 4), 4); }
-        else if (lane < 6 + MR) s_absmax[lane - 6] = 0u;
+        // one barrier per lane and round instead of ~60 serial initialisations by one thread
+        // W_EMPTY: the eight decode warps of the unit's group, after their MMAs have read the weights' digit tile
+        for (int s = lane; s < S; s += 32) { mbar_init(W_FULL(s), 1); mbar_init(X_FULL(s), 1); mbar_init(W_EMPTY(s), TC_DEC_WARPS / I8_DEC_GROUPS); }
+        if (lane < 2) { mbar_init(D_FULL(lane), TC_DEC_WARPS); mbar_init(D_EMPTY(lane), 4); }
+        else if (lane < 2 + MR) s_absmax[lane - 2] = 0u;
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<512>(smem_u32(tmem_slot));
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (threadIdx.x == 0) stamp(1);
 
     const int KB = p.k / 128;
@@ -320,12 +292,8 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     {
         // =========================== producer ===========================
         const void* tm = tmap_w;
-        // EXL3B_I8_ROWCOPY (experiment, measured slower: profiles/r02_notes.md 5): weights as eight row copies per unit instead of one
-        // 2-D tensor-map box -- 1 = multi-matrix launches, 2 = every launch, 3 = fan-out launches only (their first version)
-        const bool rag = (multi && (EXL3B_I8_ROWCOPY == 1 || (EXL3B_I8_ROWCOPY == 3 && p.rag))) || EXL3B_I8_ROWCOPY == 2;
-        const uint8_t* wsrc = !rag ? nullptr : multi ? reinterpret_cast<const uint8_t*>(p.B_ptrs[mat]) : reinterpret_cast<const uint8_t*>(p.B);
         const size_t w_pitch = (size_t) (n_loc / 16) * 32 * K;               // bytes per 16-row tile row of the packed tensor
-        if (multi && !rag)
+        if (multi)
         {
             // per-CTA tensor map: the template (dims / strides / box of this shape) with matrix `mat`'s address -- and, in a fan-out
             // launch, its own width (innermost extent in 8-byte elements, row pitch in bytes)
@@ -337,7 +305,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             else tmap_patch_address(smem_u32(stm), gtm, p.B_ptrs[mat], lane);
             tm = gtm;
         }
-        else if (!multi && !rag && elect_one()) prefetch_tmap(tmap_w);
+        else if (elect_one()) prefetch_tmap(tmap_w);
         const uint64_t pol_w = policy_evict_first();
         const uint32_t w_smem0 = smem_u32(smem);
         int strip = (int) (ubeg / KB), kb = (int) (ubeg % KB);
@@ -345,16 +313,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         for (int u = 0; u < n_units; ++u)
         {
             if (u >= S) { I8_WAITCNT(wf_a, W_EMPTY(s), ph ^ 1); mbar_wait<64>(W_EMPTY(s), ph ^ 1); }
-            if (rag)
-            {
-                // the unit's 8 tile rows x 256 K bytes, one bulk copy per row (lanes 0..7), landing exactly where the 2-D box would
-                if (lane == 0) mbar_arrive_expect_tx(W_FULL(s), (uint32_t) L.w_bytes);
-                __syncwarp();
-                if (lane < 8)
-                    bulk_g2s(w_smem0 + s * L.w_bytes + lane * (256 * K), wsrc + (size_t) (kb * 8 + lane) * w_pitch + (size_t) strip * (256 * K),
-                             256 * K, W_FULL(s), pol_w);
-            }
-            else if (elect_one())
+            if (elect_one())
             {
                 mbar_arrive_expect_tx(W_FULL(s), (uint32_t) L.w_bytes);
                 tma_load_2d(w_smem0 + s * L.w_bytes, tm, strip * (32 * K), kb * 8, W_FULL(s), pol_w);
@@ -367,102 +326,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         if (lane == 0 && p.dbg) p.dbg[blockIdx.x * 64 + 56] = wf_a;
 #endif
     }
-    else if (warp == 1)
-    {
-        // =========================== MMA issuer ===========================
-        const uint32_t idesc = idesc_u8s8_s32(128, I8_NT);
-        const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint32_t x_smem0 = smem_u32(smem + L.off_b);
-        // descriptor: K-adjacent core matrices 128 B apart (LBO), row groups 4096 B (SBO); only the 14-bit start address
-        // (16-byte units) changes: + b_bytes / 16 per stage, + 16 per MMA (256 B = 32 K-bytes x 8 rows)
-        const uint64_t desc0 = smem_desc(x_smem0, 128, 4096, 0);
-        const uint32_t desc_hi = (uint32_t) (desc0 >> 32);
-        const uint32_t desc_lo0 = (uint32_t) desc0;
-        const uint32_t desc_step = (uint32_t) (L.b_bytes >> 4);
-        uint32_t desc_lo = desc_lo0;
-        int dbuf = 0, dphase = 0, seg_left = 0, sub_left = 0;
-        uint32_t acc = 0;
-        int tsum = 0, tload = 0;                                   // lane r < m: digit sum of row r over the sub-segment
-        int kb = (int) (ubeg % KB);
-        int s = 0, sph = 0, as = 0, aph = 0;
-        for (int u = 0; u < n_units; ++u)
-        {
-            if (seg_left == 0)
-            {
-                const int to_strip_end = KB - kb;
-                seg_left = (n_units - u) < to_strip_end ? (n_units - u) : to_strip_end;
-            }
-            if (sub_left == 0)
-            {
-                sub_left = seg_left < I8_SUB_UNITS ? seg_left : I8_SUB_UNITS;
-                mbar_wait(D_EMPTY(dbuf), dphase ^ 1);
-                acc = 0;
-                tsum = 0; tload = 0;
-            }
-#ifdef EXL3B_TC_DEBUG
-            const bool mst = lane == 0 && u >= 8 && u < 12 && p.dbg;
-            if (mst) stamp(32 + 4 * (u - 8));
-#endif
-            // (the activation digits of this unit are complete too: the decode group's lead warp waited for X_FULL
-            // before it arrived here -- one barrier round trip less on this warp's serial path)
-            I8_WAITCNT(wf_b, A_FULL(as), aph);
-            mbar_wait(A_FULL(as), aph);
-            tc_fence_after();
-#ifdef EXL3B_TC_DEBUG
-            if (mst) stamp(34 + 4 * (u - 8));
-#endif
-            tsum += tload;                                              // previous unit's load: consumed one iteration late
-            if (lane < p.m) tload = *reinterpret_cast<const int*>(smem + L.off_b + s * L.b_bytes + I8_B_BYTES + 4 * lane);
-            const uint32_t d_addr = tb + I8_D_COL0 + dbuf * I8_NT;
-            uint32_t a_addr = tb + as * I8_A_STAGE_COLS;
-            --seg_left; --sub_left;
-            if (sub_left == 0)
-            {
-                tsum += tload; tload = 0;
-                if (lane < p.m) s_tout[dbuf * MR + lane] = tsum;      // visible to the epilogue before D_FULL fires
-                __threadfence_block();
-                __syncwarp();
-            }
-            if (elect_one())
-            {
-                if (!(KNOB & 4))
-                {
-                    uint32_t dl = desc_lo;
-                    #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                    {
-                        mma_i8_ts_step<8, 16>(d_addr, a_addr, dl, desc_hi, idesc, acc);
-                        acc = 1;
-#if EXL3B_I8_HALF_STAGE
-                        if (j == 7) tc_commit(A_EMPTY(as));              // columns 0..63 (tiles 0..3) are free again
-#endif
-                    }
-                }
-#if EXL3B_I8_HALF_STAGE
-                tc_commit(A_EMPTY_HI(as));
-#else
-                tc_commit(A_EMPTY(as));
-#endif
-                tc_commit(W_EMPTY(s));
-                if (sub_left == 0) tc_commit(D_FULL(dbuf));
-            }
-            acc = 1;
-            __syncwarp();
-#ifdef EXL3B_TC_DEBUG
-            if (mst) stamp(35 + 4 * (u - 8));
-#endif
-            if (sub_left == 0) { dbuf ^= 1; if (dbuf == 0) dphase ^= 1; }
-            if (++kb == KB) kb = 0;
-            desc_lo += desc_step;
-            if (++s == S) { s = 0; sph ^= 1; desc_lo = desc_lo0; }
-            if (++as == I8_A_STAGES) { as = 0; aph ^= 1; }
-        }
-        __syncwarp();
-#ifdef EXL3B_TC_DEBUG
-        if (lane == 0 && p.dbg) { p.dbg[blockIdx.x * 64 + 57] = wf_a; p.dbg[blockIdx.x * 64 + 58] = wf_b; }
-#endif
-    }
-    else if (warp < TC_DEC_WARP0)
+    else if (warp >= TC_XF_WARP0 && warp < TC_DEC_WARP0)
     {
         // =========================== activation digits (per unit) ===========================
         const int xw = warp - TC_XF_WARP0;
@@ -503,10 +367,15 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                     {
                         i8_digits(v[e], inv_scale[r], qs, hi_w[e], lo_w[e]);     // digits replicated over the 4 product bytes
                     }
-                    // chunk = lane (4 k-values x 4 bytes = 16 B), N-rows 2r (hi) and 2r+1 (lo): row group r / 4, local rows 2 (r % 4), +1
-                    uint8_t* drow = dst + (r >> 2) * 4096 + (lane * 8 + 2 * (r & 3)) * 16;
-                    *reinterpret_cast<uint4*>(drow) = make_uint4(hi_w[0], hi_w[1], hi_w[2], hi_w[3]);
-                    *reinterpret_cast<uint4*>(drow + 16) = make_uint4(lo_w[0], lo_w[1], lo_w[2], lo_w[3]);
+                    // k = 4 lane + e: K-chunk 16 (lane / 16) + 4 (lane % 4) + e, byte 4 ((lane / 4) % 4); N-rows 2r (hi) and
+                    // 2r+1 (lo): row group r / 4, local rows 2 (r % 4), +1
+                    uint8_t* drow = dst + (r >> 2) * 4096 + ((16 * (lane >> 4) + 4 * (lane & 3)) * 8 + 2 * (r & 3)) * 16 + 4 * ((lane >> 2) & 3);
+                    #pragma unroll
+                    for (int e = 0; e < 4; ++e)
+                    {
+                        *reinterpret_cast<uint32_t*>(drow + e * 128) = hi_w[e];
+                        *reinterpret_cast<uint32_t*>(drow + e * 128 + 16) = lo_w[e];
+                    }
                     qsum[r] = qs;
                 }
             }
@@ -534,109 +403,101 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         if (xw == 0 && lane == 0 && p.dbg) p.dbg[blockIdx.x * 64 + 61] = wf_a;
 #endif
     }
-    else if (warp < TC_EPI_WARP0)
+    else if (warp >= TC_DEC_WARP0 && warp < TC_EPI_WARP0)
     {
-        // =========================== decode ===========================
-        // Two groups of eight warps (three 128-column TMEM operand stages only allow two units in decode at a time);
-        // group g owns the units u = g (mod 2); inside a group the two warps of a lane quarter take alternate k-tiles.
-        const int q = warp & 3, wi = (warp - TC_DEC_WARP0) >> 2;         // wi = 0..3
-        const int g = wi & 1, sub = wi >> 1;
-        const int tl = strip_tile(q, lane), chunk = lane & 7;
-        const int prev_lane = (lane & ~7) | ((lane + 7) & 7);
-        const uint32_t lane_base = (uint32_t) (q * 32) << 16;
-        int s = g % S, sph = 0, as = g % I8_A_STAGES, aph = 0;
-        [[maybe_unused]] bool have_w = false;                                  // EXL3B_I8_PREFETCH: w already holds this unit's words
-        uint32_t w[4][K + 1];
-        for (int u = g; u < n_units; u += I8_DEC_GROUPS)
+        // =========================== decode + MMA ===========================
+        // Warpgroup (g, nh): units u = g (mod 2), output columns 64 nh .. 64 nh + 63 of the strip.  Both groups walk the same
+        // sub-segment boundaries and hand over (possibly zero) accumulators at every boundary; the epilogue adds the two.
+        const int wq = warp & 3, wgi = (warp - TC_DEC_WARP0) >> 2;
+        const int g = wgi & 1, nh = wgi >> 1;
+        const int tl = 4 * nh + wq;                      // tile column of the strip owned by this warp
+        const int chunk = lane >> 2, c = lane & 3;
+        const uint64_t desc0 = smem_desc(smem_u32(smem + L.off_b), 128, 4096, 0);
+        uint32_t acc[MR];
+        #pragma unroll
+        for (int i = 0; i < MR; ++i) acc[i] = 0u;
+        int t_lo = 0, t_hi = 0;                          // digit sums of activation rows c and c + 4 over the group's units
+        int s = 0, sph = 0, dbuf = 0, dphase = 0, seg_left = 0, sub_left = 0;
+        int kb = (int) (ubeg % KB);
+        for (int u = 0; u < n_units; ++u)
         {
-#ifdef EXL3B_TC_DEBUG
-            const bool st_on = warp == TC_DEC_WARP0 && lane == 0 && (u == 8 || u == 10) && p.dbg;
-            const int st0 = 16 + (u == 10 ? 8 : 0);
-#define I8_STAMP(i) if (st_on) stamp(st0 + (i))
-#else
-#define I8_STAMP(i)
-#endif
-            I8_STAMP(0);
-#if EXL3B_I8_PREFETCH
-            if (!have_w)
-#endif
+            if (seg_left == 0)
             {
-                I8_WAITCNT(wf_a, W_FULL(s), sph);
+                const int to_strip_end = KB - kb;
+                seg_left = (n_units - u) < to_strip_end ? (n_units - u) : to_strip_end;
+            }
+            if (sub_left == 0) sub_left = seg_left < I8_SUB_UNITS ? seg_left : I8_SUB_UNITS;
+            if ((u & 1) == g)
+            {
                 mbar_wait<32>(W_FULL(s), sph);
-                I8_STAMP(1);
                 if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) stamp(3);
                 const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
-                tc_load_tiles4<K>(wst, tl, chunk, prev_lane, sub, 2, w);           // tiles sub, sub+2, sub+4, sub+6
-            }
-            I8_STAMP(2);
-            I8_WAITCNT(wf_b, A_EMPTY(as), aph ^ 1);
-            mbar_wait(A_EMPTY(as), aph ^ 1);
-            tc_fence_after();
-            I8_STAMP(3);
-            #pragma unroll
-            for (int j = 0; j < 4; ++j)
-            {
-#if EXL3B_I8_HALF_STAGE
-                if (j == 2) { mbar_wait(A_EMPTY_HI(as), aph ^ 1); tc_fence_after(); }     // tiles 4..7 live in the stage's second half
-#endif
-                const int t = sub + 2 * j;
-                uint32_t o[16];
-                if (KNOB & 1)
+                uint32_t w[2][K + 1];
+                #pragma unroll
+                for (int r = 0; r < 2; ++r) load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, w[r]);
+                mbar_wait(X_FULL(s), sph);                                   // the unit's activation digits
+                const int* dsum = reinterpret_cast<const int*>(smem + L.off_b + s * L.b_bytes + I8_B_BYTES);
+                if (c < p.m) t_lo += dsum[c];
+                if (MR > 4 && c + 4 < p.m) t_hi += dsum[c + 4];
+                const uint64_t desc_s = desc0 + (uint64_t) ((s * L.b_bytes) >> 4);
+                #pragma unroll
+                for (int r = 0; r < 2; ++r)
                 {
+                    uint32_t o0[16], o1[16];
+                    decode16_i8<K, 0>(w[r], o0);
+                    decode16_i8<K, 1>(w[r], o1);
                     #pragma unroll
-                    for (int i = 0; i < 16; ++i) o[i] = w[j][i % (K + 1)];
+                    for (int i = 0; i < MR; ++i) reg_fence(acc[i]);
+                    wgmma_fence();
+                    #pragma unroll
+                    for (int j = 0; j < 8; ++j)
+                        wgmma_u8s8<MR>(acc, o0[2 * j], o1[2 * j], o0[2 * j + 1], o1[2 * j + 1], desc_s + (uint64_t) (16 * (8 * r + j)));
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    #pragma unroll
+                    for (int i = 0; i < 16; ++i) { reg_fence(o0[i]); reg_fence(o1[i]); }
+                    #pragma unroll
+                    for (int i = 0; i < MR; ++i) reg_fence(acc[i]);
                 }
-#if EXL3B_I8_K4_BRANCHFREE
-                else if constexpr (K == 4) decode16_i8_k4_rt(w[j], (q & 1) ? 0u : 16u, o);
-#endif
-                else if (q & 1) decode16_i8<K, 1>(w[j], o); else decode16_i8<K, 0>(w[j], o);
-                if (!(KNOB & 2))
-                    tmem_st_32x32b_x16(tmem_base + lane_base + as * I8_A_STAGE_COLS + 16 * t, o);
-                else if (o[0] == 0x12345678u && o[15] == 0x9abcdef0u) p.counters[0] = 1;
+                __syncwarp();
+                if (lane == 0) mbar_arrive(W_EMPTY(s));
+                if (u == n_units - 1 && wq == 0 && lane == 0) stamp(10);
             }
-            I8_STAMP(4);
-#if EXL3B_I8_PREFETCH
+            --seg_left; --sub_left;
+            if (sub_left == 0)
             {
-                // the next unit of this group: ring stage s + 2.  If its weights have landed, fetch its words now: the LDS /
-                // shuffle latency then overlaps the drain of the tcgen05.st above instead of opening the next unit.
-                have_w = false;
-                if (u + I8_DEC_GROUPS < n_units)
+                // hand the sub-segment's accumulators to the epilogue
+                mbar_wait(D_EMPTY(dbuf), dphase ^ 1);
+                int32_t* dst = s_d + (size_t) ((dbuf * 2 + g) * 128 + 64 * nh + 16 * wq + chunk) * (2 * MR);
+                #pragma unroll
+                for (int i = 0; i < MR / 4; ++i)
                 {
-                    int s2 = s + I8_DEC_GROUPS, sph2 = sph;
-                    if (s2 >= S) { s2 -= S; sph2 ^= 1; }
-                    if (__all_sync(0xffffffffu, mbar_test_wait(W_FULL(s2), sph2)))
-                    {
-                        const uint32_t* wst2 = reinterpret_cast<const uint32_t*>(smem + s2 * L.w_bytes);
-                        tc_load_tiles4<K>(wst2, tl, chunk, prev_lane, sub, 2, w);
-                        have_w = true;
-                    }
+                    *reinterpret_cast<int2*>(dst + 8 * i + 2 * c) = make_int2((int) acc[4 * i], (int) acc[4 * i + 1]);
+                    *reinterpret_cast<int2*>(dst + 8 * (2 * MR) + 8 * i + 2 * c) = make_int2((int) acc[4 * i + 2], (int) acc[4 * i + 3]);
                 }
+                if (nh == 0 && wq == 0 && lane < 4)
+                {
+                    s_dt[(dbuf * 2 + g) * 8 + c] = t_lo;
+                    s_dt[(dbuf * 2 + g) * 8 + c + 4] = t_hi;
+                }
+                #pragma unroll
+                for (int i = 0; i < MR; ++i) acc[i] = 0u;
+                t_lo = 0; t_hi = 0;
+                __syncwarp();
+                if (lane == 0) mbar_arrive(D_FULL(dbuf));
+                dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
             }
-#endif
-            tc_wait_st();
-            I8_STAMP(5);
-            tc_fence_before();
-            if (sub == 0 && q == 0) mbar_wait(X_FULL(s), sph);      // lead warp of the group vouches for the activation digits
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(A_FULL(as)); mbar_arrive(W_EMPTY(s)); }
-            I8_STAMP(6);
-            if (warp == TC_DEC_WARP0 && lane == 0 && u == 0) stamp(4);
-            if (q == 0 && sub == 0 && lane == 0 && u == n_units - 1) stamp(10);
-            s += I8_DEC_GROUPS; if (s >= S) { s -= S; sph ^= 1; }
-            as += I8_DEC_GROUPS; if (as >= I8_A_STAGES) { as -= I8_A_STAGES; aph ^= 1; }
+            if (++kb == KB) kb = 0;
+            if (++s == S) { s = 0; sph ^= 1; }
         }
-#ifdef EXL3B_TC_DEBUG
-        if (warp == TC_DEC_WARP0 && lane == 0 && p.dbg) { p.dbg[blockIdx.x * 64 + 59] = wf_a; p.dbg[blockIdx.x * 64 + 60] = wf_b; }
-#endif
     }
-    else
+    else if (warp >= TC_EPI_WARP0)
     {
         // =========================== epilogue ===========================
         pdl_wait();
         const int q = warp & 3;
         const int et = threadIdx.x - TC_EPI_WARP0 * 32;
-        const int col = strip_col(q, lane);
-        const uint32_t lane_base = (uint32_t) (q * 32) << 16;
+        const int col = et;                              // column of the strip this thread finishes
         float* tile = reinterpret_cast<float*>(smem + L.off_tile);
         auto epi_bar = [] { asm volatile("bar.sync 1, 128;" ::: "memory"); };
         const int part_stride = MR * 128;
@@ -787,25 +648,22 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             {
                 const int sub = (seg - done) < I8_SUB_UNITS ? (seg - done) : I8_SUB_UNITS;
                 mbar_wait<32>(D_FULL(dbuf), dphase);
-                tc_fence_after();
                 if (et == 0 && u + seg >= n_units) stamp(7);
-                uint32_t rr[16];
-                tmem_ld_32x32b_x16(tmem_base + lane_base + I8_D_COL0 + dbuf * I8_NT, rr);
-                tc_wait_ld();
+                const int32_t* d0 = s_d + (size_t) ((dbuf * 2 + 0) * 128 + col) * (2 * MR);
+                const int32_t* d1 = s_d + (size_t) ((dbuf * 2 + 1) * 128 + col) * (2 * MR);
                 #pragma unroll
                 for (int r = 0; r < MR; ++r)
                 {
                     if (r < p.m)
                     {
-                        const int T = s_tout[dbuf * MR + r];
-                        // sum_k q_k (bytesum_kn - 510), exact in 64-bit
-                        const long long sp = i8_centred_sum((int) rr[2 * r], (int) rr[2 * r + 1], T);
+                        const int T = s_dt[(dbuf * 2 + 0) * 8 + r] + s_dt[(dbuf * 2 + 1) * 8 + r];
+                        // sum_k q_k (bytesum_kn - 510), exact in 64-bit (the two groups' int32 partials add without loss)
+                        const long long sp = i8_centred_sum(d0[2 * r] + d1[2 * r], d0[2 * r + 1] + d1[2 * r + 1], T);
                         const float mx = __uint_as_float(s_absmax[r]);
                         const float scale = mx / (float) I8_QMAX;
                         facc[r] += i8_assemble(sp, T, scale, k_inv, c1);
                     }
                 }
-                tc_fence_before();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(D_EMPTY(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
@@ -895,14 +753,6 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             u += seg;
         }
         if (et == 0) stamp(8);
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1)
-    {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem_base);
     }
 }
 

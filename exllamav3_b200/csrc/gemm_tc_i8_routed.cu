@@ -1,6 +1,6 @@
 // Routed / weighted exl3_mgemm (the reference's MoE decode calls, modules/block_sparse_mlp.py:1362-1421,1435-1493: gate and up
 // with `indices` = the token's selected experts and one broadcast input, down with per-slot inputs and `weights`, optionally an
-// expert-range filter for expert-parallel shards) on the tcgen05 kind::i8 decode-GEMM (tag 212).
+// expert-range filter for expert-parallel shards) on the wgmma u8 x s8 decode-GEMM (tag 212).
 //
 //   launch 1   mgemm_resolve_kernel (gemm_simt.cu): indices / filter -> table of active slots {matrix, weight}
 //   launch 2   gemm_tc_i8_body<K, 4, false, ROUTED = true>: one CTA group per SLOT; group z runs matrix tab.mat[z] on input
@@ -10,7 +10,7 @@
 // It replaces the CUDA-core contraction that the default path (launch_mgemm, tag 100) runs between the same two bookkeeping
 // kernels; semantics are those of exl3_gemm.cu:341-381.
 //
-// STATUS: verified on a B200 in round 2 (tests/test_moe_routed.py: five routing modes vs the oracle and vs the CUDA-core twin,
+// Tests: tests/test_moe_routed.py (five routing modes vs the oracle and vs the CUDA-core twin,
 // Mixtral expert shapes); selected automatically for routed mul1 calls at <= 4 rows, the CUDA-core kernels take the rest.
 #include "gemm_tc_i8_body.cuh"
 

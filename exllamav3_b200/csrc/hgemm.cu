@@ -1,7 +1,7 @@
 // Dense fp16 GEMM  c = a @ b  (row-major, fp32 accumulate) -- replaces the reference's cuBLAS call
 // (exllamav3_ext/hgemm.cu:19-102) on the reconstruct -> hgemm prefill path.
 //
-// Dispatch: the tcgen05 kernel (hgemm_tc.cu) for 16-byte-aligned operands; this shared-memory tiled CUDA-core kernel
+// Dispatch: the wgmma kernel (hgemm_tc.cu) for 16-byte-aligned operands; this shared-memory tiled CUDA-core kernel
 // only for shapes TMA cannot address (k, n or the C row pitch not a multiple of 8).
 #include "common.cuh"
 

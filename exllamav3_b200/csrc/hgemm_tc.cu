@@ -1,12 +1,10 @@
-// Dense fp16 GEMM on tcgen05 for the reconstruct -> hgemm prefill path:  C[m,n] = A[m,k] @ B[k,n], fp32 accumulate.
+// Dense fp16 GEMM on wgmma for the reconstruct -> hgemm prefill path:  C[m,n] = A[m,k] @ B[k,n], fp32 accumulate.
 // Replaces the reference's cuBLAS call (exllamav3_ext/hgemm.cu:19-102); no library GEMM is used.
 //
-//   * persistent CTAs, one 128(m) x 256(n) output tile at a time, K in steps of 64
-//   * warp 0: TMA producer (A box 128 x 64 K-major, B as four 64(k) x 64(n) boxes, both 128-byte swizzled) into a
-//     4-stage mbarrier ring;  warp 1: TMEM allocation + single-thread tcgen05.mma.kind::f16 issue (M=128, N=256, K=16,
-//     A K-major / B MN-major straight from the row-major operands, no transposes);  warps 4-7: epilogue
-//     (tcgen05.ld 32 columns at a time -> convert -> 16-byte row stores), overlapped with the next tile's MMAs through
-//     two TMEM accumulator buffers (2 x 256 columns = all of TMEM)
+//   * persistent CTAs, one 128(m) x 128(n) output tile at a time, K in steps of 64
+//   * warp 0: TMA producer (A box 128 x 64 K-major, B as two 64(k) x 64(n) boxes, both 128-byte swizzled) into a 4-stage
+//     mbarrier ring;  warpgroups 1-2: wgmma.m64n128k16 (A K-major / B MN-major straight from the row-major operands, no
+//     transposes), 64 rows each, accumulators in registers, then convert -> masked stores from the fragments
 //   * ragged m / n / k: TMA zero-fills out-of-bounds operand elements, stores are masked
 #include "tc_common.cuh"
 #include <unordered_map>
@@ -16,10 +14,10 @@ namespace exl3b {
 
 using namespace ptx;
 
-constexpr int HG_BM = 128, HG_BN = 256, HG_BK = 64, HG_STAGES = 4;
+constexpr int HG_BM = 128, HG_BN = 128, HG_BK = 64, HG_STAGES = 4;
 constexpr int HG_A_BYTES = HG_BM * HG_BK * 2;          // 16 KB
-constexpr int HG_B_BYTES = HG_BK * HG_BN * 2;          // 32 KB
-constexpr int HG_THREADS = 256;
+constexpr int HG_B_BYTES = HG_BK * HG_BN * 2;          // 16 KB
+constexpr int HG_THREADS = 384;
 
 struct HgParams
 {
@@ -30,16 +28,25 @@ struct HgParams
     int tiles_m, tiles_n, k_iters;
 };
 
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32])
+// D[64 x 128] (f32) (+)= A[64 x 16] (f16, K-major, shared memory) * B[16 x 128] (f16, MN-major, shared memory)
+__device__ __forceinline__ void wgmma_hg(float (&d)[64], uint64_t a_desc, uint64_t b_desc, int accumulate)
 {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
                  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr) : "memory");
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+                 "%64, %65, p, 1, 1, 0, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
 }
 
 __global__ void __launch_bounds__(HG_THREADS, 1)
@@ -48,376 +55,97 @@ hgemm_tc_kernel(const HgParams p, const __grid_constant__ CUtensorMap tmA, const
     extern __shared__ __align__(1024) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint8_t* sA = smem;                                   // HG_STAGES x 16 KB
-    uint8_t* sB = smem + HG_STAGES * HG_A_BYTES;          // HG_STAGES x 32 KB
+    uint8_t* sB = smem + HG_STAGES * HG_A_BYTES;          // HG_STAGES x 16 KB
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + HG_STAGES * (HG_A_BYTES + HG_B_BYTES));
     const uint32_t bar0 = smem_u32(bars);
     auto FULL = [&](int s) { return bar0 + 8u * s; };
     auto EMPTY = [&](int s) { return bar0 + 8u * (HG_STAGES + s); };
-    auto D_FULL = [&](int s) { return bar0 + 8u * (2 * HG_STAGES + s); };
-    auto D_EMPTY = [&](int s) { return bar0 + 8u * (2 * HG_STAGES + 2 + s); };
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * HG_STAGES + 4);
 
     if (threadIdx.x == 0)
     {
-        for (int s = 0; s < HG_STAGES; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(D_FULL(s), 1); mbar_init(D_EMPTY(s), 4); }
+        for (int s = 0; s < HG_STAGES; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 8); }     // EMPTY: the 8 consumer warps
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<512>(smem_u32(tmem_slot));
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    const int n_tiles = p.tiles_m * p.tiles_n;
+    const int tiles = p.tiles_m * p.tiles_n;
 
     if (warp == 0)
     {
         // =========================== TMA producer ===========================
         if (elect_one()) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-        const uint64_t pol = policy_evict_last();          // both operands are re-read by other CTAs: keep them in L2
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-        int s = 0, ph = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x)
+        const uint64_t pol = policy_evict_last();
+        int s = 0, ph = 0, it = 0;
+        for (int t = blockIdx.x; t < tiles; t += gridDim.x)
         {
-            const int mb = t / p.tiles_n, nb = t % p.tiles_n;
-            for (int ki = 0; ki < p.k_iters; ++ki)
+            const int tm = t / p.tiles_n, tn = t - tm * p.tiles_n;
+            for (int ki = 0; ki < p.k_iters; ++ki, ++it)
             {
-                mbar_wait<32>(EMPTY(s), ph ^ 1);
+                if (it >= HG_STAGES) mbar_wait<64>(EMPTY(s), ph ^ 1);
                 if (elect_one())
                 {
                     mbar_arrive_expect_tx(FULL(s), HG_A_BYTES + HG_B_BYTES);
-                    tma_load_2d(a0 + s * HG_A_BYTES, &tmA, ki * HG_BK, mb * HG_BM, FULL(s), pol);
+                    tma_load_2d(smem_u32(sA + s * HG_A_BYTES), &tmA, ki * HG_BK, tm * HG_BM, FULL(s), pol);
                     #pragma unroll
-                    for (int j = 0; j < 4; ++j)
-                        tma_load_2d(b0 + s * HG_B_BYTES + j * 8192, &tmB, nb * HG_BN + j * 64, ki * HG_BK, FULL(s), pol);
+                    for (int j = 0; j < HG_BN / 64; ++j)
+                        tma_load_2d(smem_u32(sB + s * HG_B_BYTES + j * 8192), &tmB, tn * HG_BN + 64 * j, ki * HG_BK, FULL(s), pol);
                 }
-                if (++s == HG_STAGES) { s = 0; ph ^= 1; }
-            }
-        }
-        __syncwarp();
-    }
-    else if (warp == 1)
-    {
-        // =========================== MMA issuer ===========================
-        const uint32_t idesc = idesc_f16_f32(HG_BM, HG_BN, /*b_mn_major=*/true);
-        const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-        // A: K-major, 128-byte swizzle: 8-row groups 1024 B apart (SBO); LBO unused (1)
-        const uint64_t descA = smem_desc(0, 16, 1024, 2);
-        // B: MN-major, 128-byte swizzle: 64-column blocks 8192 B apart (LBO), 8-row K groups 1024 B apart (SBO)
-        const uint64_t descB = smem_desc(0, 8192, 1024, 2);
-        int s = 0, ph = 0, dbuf = 0, dph = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x)
-        {
-            mbar_wait(D_EMPTY(dbuf), dph ^ 1);
-            uint32_t acc = 0;
-            for (int ki = 0; ki < p.k_iters; ++ki)
-            {
-                mbar_wait(FULL(s), ph);
-                tc_fence_after();
-                if (elect_one())
-                {
-                    const uint32_t a_addr = a0 + s * HG_A_BYTES, b_addr = b0 + s * HG_B_BYTES;
-                    #pragma unroll
-                    for (int kk = 0; kk < HG_BK / 16; ++kk)
-                    {
-                        const uint64_t da = descA | (uint64_t) (((a_addr + kk * 32) >> 4) & 0x3fff);
-                        const uint64_t db = descB | (uint64_t) (((b_addr + kk * 2048) >> 4) & 0x3fff);
-                        mma_f16_ss(tb + dbuf * HG_BN, da, db, idesc, acc);
-                        acc = 1;
-                    }
-                    tc_commit(EMPTY(s));
-                    if (ki == p.k_iters - 1) tc_commit(D_FULL(dbuf));
-                }
-                acc = 1;
                 __syncwarp();
                 if (++s == HG_STAGES) { s = 0; ph ^= 1; }
             }
-            dbuf ^= 1; if (dbuf == 0) dph ^= 1;
         }
-        __syncwarp();
     }
     else if (warp >= 4)
     {
-        // =========================== epilogue ===========================
-        const int q = warp & 3;
-        const uint32_t lane_base = (uint32_t) (q * 32) << 16;
-        int dbuf = 0, dph = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x)
-        {
-            const int mb = t / p.tiles_n, nb = t % p.tiles_n;
-            const int row = mb * HG_BM + q * 32 + lane;
-            mbar_wait<32>(D_FULL(dbuf), dph);
-            tc_fence_after();
-            #pragma unroll 1
-            for (int c = 0; c < HG_BN / 32; ++c)
-            {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(tmem_base + lane_base + dbuf * HG_BN + c * 32, r);
-                tc_wait_ld();
-                const int col0 = nb * HG_BN + c * 32;
-                if (row < p.m && col0 < p.n)
-                {
-                    if (p.c_fp32)
-                    {
-                        float* dst = (float*) p.C + (size_t) row * p.c_stride + col0;
-                        #pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            if (col0 + 4 * j < p.n)
-                                *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                                                                   __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
-                    }
-                    else
-                    {
-                        half* dst = (half*) p.C + (size_t) row * p.c_stride + col0;
-                        #pragma unroll
-                        for (int j = 0; j < 4; ++j)
-                        {
-                            if (col0 + 8 * j < p.n)
-                            {
-                                uint4 o;
-                                half2 h;
-                                h = __floats2half2_rn(__uint_as_float(r[8 * j + 0]), __uint_as_float(r[8 * j + 1])); o.x = *reinterpret_cast<uint32_t*>(&h);
-                                h = __floats2half2_rn(__uint_as_float(r[8 * j + 2]), __uint_as_float(r[8 * j + 3])); o.y = *reinterpret_cast<uint32_t*>(&h);
-                                h = __floats2half2_rn(__uint_as_float(r[8 * j + 4]), __uint_as_float(r[8 * j + 5])); o.z = *reinterpret_cast<uint32_t*>(&h);
-                                h = __floats2half2_rn(__uint_as_float(r[8 * j + 6]), __uint_as_float(r[8 * j + 7])); o.w = *reinterpret_cast<uint32_t*>(&h);
-                                *reinterpret_cast<uint4*>(dst + 8 * j) = o;
-                            }
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(D_EMPTY(dbuf));
-            dbuf ^= 1; if (dbuf == 0) dph ^= 1;
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1)
-    {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem_base);
-    }
-}
-
-// =====================================================================================================================
-// Two-CTA variant (cta_group::2): a CTA pair (one TPC) computes a 256(m) x 256(n) tile.  Each CTA stages its own 128 rows of A
-// and HALF of the B tile (128 of the 256 columns); tcgen05.mma.cta_group::2 (M = 256), issued by the pair's leader, reads both
-// CTAs' shared memory, so every B byte is fetched from L2 and written to shared memory once per pair instead of once per CTA:
-// per CTA and k-step 32 KB of TMA traffic instead of 48 KB, and six ring stages instead of four in the same shared memory.
-//   barriers: FULL lives in the leader (both CTAs' TMA loads complete_tx on it, the leader expects the pair's bytes);
-//   EMPTY / D_FULL exist in both CTAs and are signalled by the leader's tcgen05.commit with a 2-CTA multicast mask;
-//   D_EMPTY lives in the leader and counts the epilogue warps of both CTAs (remote mbarrier.arrive).
-// =====================================================================================================================
-constexpr int HG2_STAGES = 6;
-constexpr int HG2_A_BYTES = 128 * HG_BK * 2;           // 16 KB: this CTA's 128 rows
-constexpr int HG2_B_BYTES = HG_BK * 128 * 2;           // 16 KB: this CTA's 128 of the tile's 256 columns
-constexpr uint32_t HG2_PEER_MASK = 0xFEFFFFFFu;        // shared::cluster address of the same offset in the pair's even (leader) CTA
-
-__device__ __forceinline__ uint32_t cluster_ctarank()
-{
-    uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r;
-}
-__device__ __forceinline__ void cluster_sync_all()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const void* tmap, int c0, int c1, uint32_t bar_leader, uint64_t policy)
-{
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-                 " [%0], [%1, {%2, %3}], [%4], %5;"
-                 :: "r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(bar_leader), "l"(policy) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar)
-{
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" :: "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_commit_2sm(uint32_t bar, uint16_t cta_mask)
-{
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 :: "r"(bar), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ void mma_f16_ss_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\t"
-                 "setp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(HG_THREADS, 1)
-hgemm_tc2_kernel(const HgParams p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB)
-{
-    extern __shared__ __align__(1024) uint8_t smem[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    uint8_t* sA = smem;
-    uint8_t* sB = smem + HG2_STAGES * HG2_A_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + HG2_STAGES * (HG2_A_BYTES + HG2_B_BYTES));
-    const uint32_t bar0 = smem_u32(bars);
-    auto FULL = [&](int s) { return bar0 + 8u * s; };
-    auto EMPTY = [&](int s) { return bar0 + 8u * (HG2_STAGES + s); };
-    auto D_FULL = [&](int s) { return bar0 + 8u * (2 * HG2_STAGES + s); };
-    auto D_EMPTY = [&](int s) { return bar0 + 8u * (2 * HG2_STAGES + 2 + s); };
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * HG2_STAGES + 4);
-
-    if (threadIdx.x == 0)
-    {
-        for (int s = 0; s < HG2_STAGES; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(D_FULL(s), 1); mbar_init(D_EMPTY(s), 8); }      // 4 epilogue warps x 2 CTAs
-        fence_barrier_init();
-    }
-    if (warp == 1)
-    {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                   // both CTAs' barriers exist before anyone signals across the pair
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    const int tiles_m2 = (p.m + 255) / 256;
-    const int n_tiles = tiles_m2 * p.tiles_n;
-    const int cl = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-
-    if (warp == 0)
-    {
-        // =========================== TMA producer (both CTAs) ===========================
-        if (elect_one()) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-        const uint64_t pol = policy_evict_last();
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
+        // =========================== consumers: warpgroup h = rows 64 h .. 64 h + 63 of the tile ===========================
+        const int h = (warp - 4) >> 2, wq = warp & 3;
+        // A: K-major, 128-byte swizzle (8-row atoms 1024 B apart); B: MN-major, 128-byte swizzle (8-k atoms 1024 B apart,
+        // 64-column boxes 8192 B apart)
+        const uint64_t descA0 = smem_desc(smem_u32(sA) + h * 64 * 128, 16, 1024, 1);
+        const uint64_t descB0 = smem_desc(smem_u32(sB), 8192, 1024, 1);
+        const int r_in = 64 * h + 16 * wq + (lane >> 2), c2 = 2 * (lane & 3);
         int s = 0, ph = 0;
-        for (int t = cl; t < n_tiles; t += ncl)
+        for (int t = blockIdx.x; t < tiles; t += gridDim.x)
         {
-            const int mb = t / p.tiles_n, nb = t % p.tiles_n;
+            const int tm = t / p.tiles_n, tn = t - tm * p.tiles_n;
+            float d[64];
+            #pragma unroll
+            for (int i = 0; i < 64; ++i) d[i] = 0.f;
             for (int ki = 0; ki < p.k_iters; ++ki)
             {
-                mbar_wait<32>(EMPTY(s), ph ^ 1);
-                if (elect_one())
-                {
-                    const uint32_t full_leader = FULL(s) & HG2_PEER_MASK;
-                    if (leader) mbar_arrive_expect_tx(FULL(s), 2 * (HG2_A_BYTES + HG2_B_BYTES));
-                    tma_load_2d_2sm(a0 + s * HG2_A_BYTES, &tmA, ki * HG_BK, mb * 256 + (int) rank * 128, full_leader, pol);
-                    #pragma unroll
-                    for (int j = 0; j < 2; ++j)
-                        tma_load_2d_2sm(b0 + s * HG2_B_BYTES + j * 8192, &tmB, nb * HG_BN + (int) rank * 128 + j * 64, ki * HG_BK, full_leader, pol);
-                }
-                if (++s == HG2_STAGES) { s = 0; ph ^= 1; }
-            }
-        }
-        __syncwarp();
-    }
-    else if (warp == 1 && leader)
-    {
-        // =========================== MMA issuer (leader CTA only) ===========================
-        const uint32_t idesc = idesc_f16_f32(256, HG_BN, /*b_mn_major=*/true);
-        const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-        const uint64_t descA = smem_desc(0, 16, 1024, 2);
-        const uint64_t descB = smem_desc(0, 8192, 1024, 2);
-        int s = 0, ph = 0, dbuf = 0, dph = 0;
-        for (int t = cl; t < n_tiles; t += ncl)
-        {
-            mbar_wait(D_EMPTY(dbuf), dph ^ 1);
-            tc_fence_after();
-            uint32_t acc = 0;
-            for (int ki = 0; ki < p.k_iters; ++ki)
-            {
-                mbar_wait(FULL(s), ph);
-                tc_fence_after();
-                if (elect_one())
-                {
-                    const uint32_t a_addr = a0 + s * HG2_A_BYTES, b_addr = b0 + s * HG2_B_BYTES;
-                    #pragma unroll
-                    for (int kk = 0; kk < HG_BK / 16; ++kk)
-                    {
-                        const uint64_t da = descA | (uint64_t) (((a_addr + kk * 32) >> 4) & 0x3fff);
-                        const uint64_t db = descB | (uint64_t) (((b_addr + kk * 2048) >> 4) & 0x3fff);
-                        mma_f16_ss_2sm(tb + dbuf * HG_BN, da, db, idesc, acc);
-                        acc = 1;
-                    }
-                    tc_commit_2sm(EMPTY(s), 3);
-                    if (ki == p.k_iters - 1) tc_commit_2sm(D_FULL(dbuf), 3);
-                }
-                acc = 1;
+                mbar_wait<32>(FULL(s), ph);
+                #pragma unroll
+                for (int i = 0; i < 64; ++i) reg_fence(d[i]);
+                wgmma_fence();
+                #pragma unroll
+                for (int j = 0; j < HG_BK / 16; ++j)
+                    wgmma_hg(d, descA0 + (uint64_t) ((s * HG_A_BYTES + 32 * j) >> 4), descB0 + (uint64_t) ((s * HG_B_BYTES + 2048 * j) >> 4), 1);
+                wgmma_commit();
+                wgmma_wait<0>();
+                #pragma unroll
+                for (int i = 0; i < 64; ++i) reg_fence(d[i]);
                 __syncwarp();
-                if (++s == HG2_STAGES) { s = 0; ph ^= 1; }
+                if (lane == 0) mbar_arrive(EMPTY(s));
+                if (++s == HG_STAGES) { s = 0; ph ^= 1; }
             }
-            dbuf ^= 1; if (dbuf == 0) dph ^= 1;
-        }
-        __syncwarp();
-    }
-    else if (warp >= 4)
-    {
-        // =========================== epilogue (both CTAs: own 128 rows) ===========================
-        const int q = warp & 3;
-        const uint32_t lane_base = (uint32_t) (q * 32) << 16;
-        int dbuf = 0, dph = 0;
-        for (int t = cl; t < n_tiles; t += ncl)
-        {
-            const int mb = t / p.tiles_n, nb = t % p.tiles_n;
-            const int row = mb * 256 + (int) rank * 128 + q * 32 + lane;
-            mbar_wait<32>(D_FULL(dbuf), dph);
-            tc_fence_after();
-            #pragma unroll 1
-            for (int c = 0; c < HG_BN / 32; ++c)
+            // ---- epilogue from the fragments: rows r, r + 8, columns 8 j + 2c, +1 ----
+            #pragma unroll
+            for (int hr = 0; hr < 2; ++hr)
             {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(tmem_base + lane_base + dbuf * HG_BN + c * 32, r);
-                tc_wait_ld();
-                const int col0 = nb * HG_BN + c * 32;
-                if (row < p.m && col0 < p.n)
+                const int row = tm * HG_BM + r_in + 8 * hr;
+                if (row >= p.m) continue;
+                #pragma unroll
+                for (int j = 0; j < 16; ++j)
                 {
+                    const int col = tn * HG_BN + 8 * j + c2;
+                    if (col >= p.n) continue;                  // n % 8 == 0: a column pair is in or out as a whole
+                    const float v0 = d[4 * j + 2 * hr], v1 = d[4 * j + 2 * hr + 1];
                     if (p.c_fp32)
-                    {
-                        float* dst = (float*) p.C + (size_t) row * p.c_stride + col0;
-                        #pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            if (col0 + 4 * j < p.n)
-                                *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                                                                   __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
-                    }
+                        *reinterpret_cast<float2*>((float*) p.C + (size_t) row * p.c_stride + col) = make_float2(v0, v1);
                     else
-                    {
-                        half* dst = (half*) p.C + (size_t) row * p.c_stride + col0;
-                        #pragma unroll
-                        for (int j = 0; j < 4; ++j)
-                        {
-                            if (col0 + 8 * j < p.n)
-                            {
-                                uint4 o;
-                                half2 h;
-                                h = __floats2half2_rn(__uint_as_float(r[8 * j + 0]), __uint_as_float(r[8 * j + 1])); o.x = *reinterpret_cast<uint32_t*>(&h);
-                                h = __floats2half2_rn(__uint_as_float(r[8 * j + 2]), __uint_as_float(r[8 * j + 3])); o.y = *reinterpret_cast<uint32_t*>(&h);
-                                h = __floats2half2_rn(__uint_as_float(r[8 * j + 4]), __uint_as_float(r[8 * j + 5])); o.z = *reinterpret_cast<uint32_t*>(&h);
-                                h = __floats2half2_rn(__uint_as_float(r[8 * j + 6]), __uint_as_float(r[8 * j + 7])); o.w = *reinterpret_cast<uint32_t*>(&h);
-                                *reinterpret_cast<uint4*>(dst + 8 * j) = o;
-                            }
-                        }
-                    }
+                        *reinterpret_cast<half2*>((half*) p.C + (size_t) row * p.c_stride + col) = __floats2half2_rn(v0, v1);
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(D_EMPTY(dbuf) & HG2_PEER_MASK);        // the leader's barrier counts both CTAs' warps
-            dbuf ^= 1; if (dbuf == 0) dph ^= 1;
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                   // nobody frees TMEM / leaves while the peer may still use this CTA's memory
-    if (warp == 1)
-    {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "n"(512) : "memory");
     }
 }
 
@@ -452,13 +180,10 @@ static int make_tmap_fp16_2d(const void* base, uint64_t inner, uint64_t outer, u
     return 0;
 }
 
-int g_hgemm_pair = 0;
-void hgemm_set_pair_mode(int mode) { g_hgemm_pair = mode; }
-
 bool hgemm_tc_supported(const void* a, const void* b, const void* c, int m, int k, int n, int64_t c_stride)
 {
-    // TMA needs 16-byte aligned bases and row pitches; the epilogue stores 16-byte vectors.  Anything else (e.g. an
-    // unaligned view) takes the CUDA-core kernel instead of an error.
+    // TMA needs 16-byte aligned bases and row pitches.  Anything else (e.g. an unaligned view) takes the CUDA-core kernel
+    // instead of an error.
     const bool aligned = (((uintptr_t) a | (uintptr_t) b | (uintptr_t) c) & 15) == 0;
     return aligned && m >= 1 && k >= 8 && n >= 8 && k % 8 == 0 && n % 8 == 0 && c_stride % 8 == 0;
 }
@@ -483,23 +208,6 @@ int launch_hgemm_tc(cudaStream_t stream, const half* a, const half* b, void* c, 
         attr_set[dev & 31] = true;
     }
     int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // CTA pairs (cta_group::2, 256 x 256 tiles) whenever there is more than one 128-row tile; g_hgemm_pair: 0 = auto, 1 = never, 2 = always
-    if ((m > 128 && g_hgemm_pair != 1) || g_hgemm_pair == 2)
-    {
-        static bool attr2_set[32] = {};
-        const int smem2 = HG2_STAGES * (HG2_A_BYTES + HG2_B_BYTES) + 256;
-        if (!attr2_set[dev & 31])
-        {
-            EXL3B_CUDA(cudaFuncSetAttribute(hgemm_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2));
-            attr2_set[dev & 31] = true;
-        }
-        const int tiles2 = ((m + 255) / 256) * p.tiles_n;
-        int grid2 = 2 * tiles2; if (grid2 > (sms & ~1)) grid2 = sms & ~1;
-        hgemm_tc2_kernel<<<grid2, HG_THREADS, smem2, stream>>>(p, tmA, tmB);
-        count_launch();
-        EXL3B_CUDA(cudaPeekAtLastError());
-        return 0;
-    }
     int grid = p.tiles_m * p.tiles_n; if (grid > sms) grid = sms;
     hgemm_tc_kernel<<<grid, HG_THREADS, smem_bytes, stream>>>(p, tmA, tmB);
     count_launch();

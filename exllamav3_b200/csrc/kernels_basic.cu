@@ -1,4 +1,4 @@
-// had_r_128, reconstruct, reconstruct_had -- the memory-bound helpers of the EXL3 path, sm_100a.
+// had_r_128, reconstruct, reconstruct_had -- the memory-bound helpers of the EXL3 path.
 //
 // Reference behaviour restated (not copied): exllamav3_ext/quant/hadamard.cu:88-173 + hadamard_inner.cuh:93-277,
 // exllamav3_ext/quant/reconstruct.cu:11-144 (plain), :159-373 (fused both-side Hadamard).

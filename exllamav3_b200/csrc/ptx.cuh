@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features this library uses: mbarrier, bulk async copy (TMA engine,
-// SASS UBLKCP), tcgen05 (TMEM alloc / st / ld / mma / commit / fences), programmatic dependent launch.
+// Thin inline-PTX wrappers for the sm_90a features this library uses: mbarrier, bulk async copy (TMA engine,
+// SASS UBLKCP), wgmma (warpgroup MMA), programmatic dependent launch.
 #pragma once
 #include <stdint.h>
 #include <cuda_runtime.h>
@@ -8,9 +8,8 @@ namespace exl3b { namespace ptx {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t) __cvta_generic_to_shared(p); }
 
-// One elected lane of a fully converged warp.  Keeping the surrounding control flow warp-uniform lets ptxas keep TMA /
-// tcgen05 operands in uniform registers; issuing from inside an `if (lane == 0)` region instead costs a
-// R2UR "waterfall" loop of ~16 dependent instructions per UTCHMMA (measured: 56 cycles per MMA issue).
+// One elected lane of a fully converged warp.  Keeping the surrounding control flow warp-uniform lets ptxas keep TMA
+// operands in uniform registers instead of a per-lane R2UR loop.
 __device__ __forceinline__ bool elect_one()
 {
     uint32_t pred;
@@ -40,8 +39,7 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
 }
 // try_wait with a suspend-time hint: the warp sleeps in hardware until the phase completes (or the hint expires)
-// instead of polling -- polling warps (epilogue / MMA / producer roles) were measured to consume ~40 % of all issue
-// slots of the first version of the kernel (profiles/r01_ncu_tc_v1_notes.md).
+// instead of polling, so waiting warps do not take issue slots from the decode warps.
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity)
 {
     uint32_t ok;
@@ -65,8 +63,7 @@ __device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity)
 // (%globaltimer, checked every 1024 polls), not an iteration count: try_wait returns early whenever ANY barrier
 // activity wakes the warp, so iteration counts say nothing about elapsed time.
 // BACKOFF_NS > 0: exponential back-off (BACKOFF_NS, 2x, ... capped at 16x) between polls for roles whose waits can be
-// long: polling warps otherwise burn issue slots the decode warps need (measured: ~40 % of all issued instructions of
-// the first version of the kernel were polls; profiles/r01_ncu_notes.md).
+// long: polling warps otherwise burn issue slots the decode warps need.
 template <int BACKOFF_NS = 0>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
 {
@@ -197,125 +194,51 @@ __device__ __forceinline__ void st_relaxed_sys_v4(uint32_t* p, uint4 v)
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// ---- tcgen05 / TMEM ----------------------------------------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_dst), "n"(NCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after()  { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// ---- wgmma (sm_90a warpgroup MMA) -------------------------------------------------------------------------------
+// All four warps of a warpgroup (warps 4w .. 4w+3) execute these together.  The A operand comes from registers (the decode
+// threads' own decoded weights), B from shared memory through a descriptor, D lives in registers.
+// The .aligned instructions need every lane of the warp converged: lanes that left an mbarrier poll loop at different
+// iterations are joined first.
+__device__ __forceinline__ void wgmma_fence()  { __syncwarp(); asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait()   { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+// keeps the compiler from moving accesses of a register across the asynchronous MMA (or reusing it while the MMA reads it)
+__device__ __forceinline__ void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r) :: "memory"); }
+__device__ __forceinline__ void reg_fence(float& r)    { asm volatile("" : "+f"(r) :: "memory"); }
 
-// 32 lanes x 8 consecutive 32-bit columns; thread i of the warp writes TMEM lane (warp%4)*32 + i
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8])
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr) : "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem desc], kind::f16 (fp16 x fp16 -> fp32), one CTA
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\t"
-                 "setp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-                 :: "r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc], kind::i8 (8-bit integers -> int32), one CTA
-__device__ __forceinline__ void mma_i8_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\t"
-                 "setp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], %2, %3, p;\n\t}"
-                 :: "r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// same, the shared-memory descriptor given as its two 32-bit halves (lets the caller step the 14-bit start-address field
-// with one 32-bit add per instruction instead of rebuilding the 64-bit descriptor)
-__device__ __forceinline__ void mma_i8_ts_lohi(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_desc_lo, uint32_t b_desc_hi, uint32_t idesc,
-                                               uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 bd;\n\t"
-                 "setp.ne.b32 p, %5, 0;\n\t"
-                 "mov.b64 bd, {%2, %3};\n\t"
-                 "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], bd, %4, p;\n\t}"
-                 :: "r"(d_tmem), "r"(a_tmem), "r"(b_desc_lo), "r"(b_desc_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-// same, stepping the A address and the descriptor start address in place after the issue (keeps the whole unrolled MMA
-// sequence on ONE uniform-register pair instead of one pair + one high-word move per instruction)
-template <int A_STEP, int B_STEP>
-__device__ __forceinline__ void mma_i8_ts_step(uint32_t d_tmem, uint32_t& a_tmem, uint32_t& b_desc_lo, uint32_t b_desc_hi, uint32_t idesc,
-                                               uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 bd;\n\t"
-                 "setp.ne.b32 p, %5, 0;\n\t"
-                 "mov.b64 bd, {%1, %3};\n\t"
-                 "tcgen05.mma.cta_group::1.kind::i8 [%2], [%0], bd, %4, p;\n\t"
-                 "add.u32 %0, %0, %6;\n\t"
-                 "add.u32 %1, %1, %7;\n\t}"
-                 : "+r"(a_tmem), "+r"(b_desc_lo) : "r"(d_tmem), "r"(b_desc_hi), "r"(idesc), "r"(accumulate), "n"(A_STEP), "n"(B_STEP) : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16])
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-                 :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-                    "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-                 : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\t"
-                 "setp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05 async ops of this thread have completed
-__device__ __forceinline__ void tc_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(bar) : "memory");
-}
-
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): start address, leading-dimension and
-// stride-dimension byte offsets in 16-byte units, descriptor version 1 (Blackwell), layout type in bits 61..63
-// (0 = no swizzle / interleaved 8x16B core matrices, 2 = 128-byte swizzle).
+// Shared-memory matrix descriptor of wgmma: start address, leading-dimension byte offset (K-adjacent core matrices for a
+// K-major operand without swizzle, the unused 1 for a swizzled K-major one) and stride-dimension byte offset (8-row groups),
+// all in 16-byte units; layout type in bits 62..63 (0 = no swizzle / 8 x 16 B core matrices, 1 = 128-byte swizzle).
 __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type)
 {
     uint64_t d = 0;
     d |= (uint64_t) ((saddr >> 4) & 0x3fff);
     d |= (uint64_t) ((lbo_bytes >> 4) & 0x3fff) << 16;
     d |= (uint64_t) ((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= (uint64_t) 1 << 46;
-    d |= (uint64_t) (layout_type & 7) << 61;
+    d |= (uint64_t) (layout_type & 3) << 62;
     return d;
 }
 
-// Instruction descriptor for kind::f16 with fp16 A/B (format 0), fp32 accumulate (c_format 1), both K-major
-// (cute::UMMA::InstrDescriptor): n_dim = N >> 3 at bit 17, m_dim = M >> 4 at bit 24.
-__device__ __host__ __forceinline__ uint32_t idesc_f16_f32(int M, int N, bool b_mn_major = false)
+// D[64 x 8] (s32) += A[64 x 32] (u8, registers) * B[32 x 8] (s8, shared memory, K-major)
+__device__ __forceinline__ void wgmma_u8s8_n8(uint32_t (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc)
 {
-    return (1u << 4) | ((b_mn_major ? 1u : 0u) << 16) | ((uint32_t) (N >> 3) << 17) | ((uint32_t) (M >> 4) << 24);
+    asm volatile("wgmma.mma_async.sync.aligned.m64n8k32.s32.u8.s8 {%0, %1, %2, %3}, {%4, %5, %6, %7}, %8, 1;"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc) : "memory");
 }
-
-// kind::i8: A unsigned 8-bit (format 0), B signed 8-bit (format 1), int32 accumulate (c_format 2), both K-major
-__device__ __host__ __forceinline__ uint32_t idesc_u8s8_s32(int M, int N)
+// D[64 x 16] (s32) += A[64 x 32] (u8, registers) * B[32 x 16] (s8, shared memory, K-major)
+__device__ __forceinline__ void wgmma_u8s8_n16(uint32_t (&d)[8], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc)
 {
-    return (2u << 4) | (0u << 7) | (1u << 10) | ((uint32_t) (N >> 3) << 17) | ((uint32_t) (M >> 4) << 24);
+    asm volatile("wgmma.mma_async.sync.aligned.m64n16k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, 1;"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc) : "memory");
+}
+template <int MR>
+__device__ __forceinline__ void wgmma_u8s8(uint32_t (&d)[MR], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc)
+{
+    if constexpr (MR == 4) wgmma_u8s8_n8(d, a0, a1, a2, a3, b_desc);
+    else wgmma_u8s8_n16(d, a0, a1, a2, a3, b_desc);
 }
 
 }}  // namespace exl3b::ptx

@@ -1,4 +1,4 @@
-// Shared declarations of the tcgen05 kernels (exact fp16 path: gemm_tc.cu, int8 codebook path: gemm_tc_i8.cu).
+// Shared declarations of the tensor-core kernels (exact fp16 path: gemm_tc.cu, int8 codebook path: gemm_tc_i8.cu).
 #pragma once
 #include "common.cuh"
 #include "decode.cuh"
@@ -11,12 +11,10 @@ namespace exl3b {
 constexpr int TC_THREADS = 768;
 constexpr int TC_XF_WARP0 = 2;               // warps 2,3: in-kernel input transform (small m)
 constexpr int TC_DEC_WARP0 = 4;
-constexpr int TC_DEC_WARPS = 16;             // 4 per lane quarter: tiles {h, h+4} of every unit
-constexpr int TC_DEC_GROUPS = 4;             // exact path: groups of 4 warps, each owning every 4th unit
+constexpr int TC_DEC_WARPS = 16;             // four decode warpgroups
 constexpr int TC_EPI_WARP0 = TC_DEC_WARP0 + TC_DEC_WARPS;
 constexpr int TC_MAX_STAGES = 16;
 constexpr int TC_RAG_MAX_MATS = 8;          // matrices of a fan-out launch (per-matrix widths)
-constexpr int TC_A_STAGE_COLS = 64;          // 128 k-values x fp16, 2 per 32-bit TMEM column
 
 struct TcParams
 {
@@ -32,9 +30,6 @@ struct TcParams
     int stages;                  // smem ring depth
     int b_bytes;                 // bytes reserved per activation stage
     int b_load_bytes;            // bytes of the activation tile copied per unit
-    int a_stages;                // TMEM A-operand stages (3 or 4)
-    int d_bufs;                  // TMEM accumulator buffers (1 or 2)
-    int tmem_cols;               // 256 or 512
     const half* A_raw;           // fused input transform (m <= 8): raw activations (m, k) and suh; null -> xh_tiled is used
     const half* suh;
     // multi-matrix launch (exl3_mgemm, dense case): the grid is num_mats groups of g_per_mat CTAs, group j works on
@@ -52,7 +47,7 @@ struct TcParams
     const uint64_t* c_ptrs;
     float* parts;                // i8 path: sentinel-managed split-K exchange buffer (one 4 x 128 fp32 slot per CTA)
     uint8_t* tmap_slots;         // one 128-byte tensor-map slot per CTA (global memory)
-    int knob_;                   // bring-up experiment switches (0 in production): 1 skip decode math, 2 skip STTM, 4 skip MMA
+    int knob_;                   // bring-up experiment switches (0 in production)
     unsigned long long* dbg;     // optional per-CTA timeline (16 x u64 per CTA), bring-up only
 };
 
@@ -78,7 +73,7 @@ struct RouteArgs
 
 struct TcSmemLayout
 {
-    int w_bytes, b_bytes, off_b, off_tile, off_bars, total;
+    int w_bytes, b_bytes, off_b, off_tile, off_bars, off_d, total;
 };
 
 __host__ __device__ inline TcSmemLayout tc_smem_layout(int K, int b_bytes, int stages)
@@ -90,6 +85,7 @@ __host__ __device__ inline TcSmemLayout tc_smem_layout(int K, int b_bytes, int s
     L.off_tile = L.off_b + stages * L.b_bytes;
     L.off_bars = L.off_tile + 16 * 128 * 4;
     L.total = L.off_bars + 1024;
+    L.off_d = L.total;
     return L;
 }
 
@@ -98,45 +94,6 @@ __host__ __device__ inline TcSmemLayout tc_smem_layout(int K, int b_bytes, int s
 __host__ __device__ __forceinline__ long long unit_begin(long long U, int G, int c) { return U * c / G; }
 __host__ __device__ __forceinline__ int cta_of_unit(long long U, int G, long long g) { return (int) (((g + 1) * G - 1) / U); }
 
-
-// Load the K+1 words (chunk + preceding word, the latter by shuffle from the neighbouring lane) of four tiles
-// t0, t0 + tstride, ... of this lane's (tile-in-strip, chunk) from a weight stage in shared memory.
-template <int K>
-__device__ __forceinline__ void tc_load_tiles4(const uint32_t* wst, int tl, int chunk, int prev_lane, int t0, int tstride,
-                                               uint32_t (&w)[4][K + 1])
-{
-    #pragma unroll
-    for (int j = 0; j < 4; ++j)
-    {
-        const uint32_t* cp = wst + ((t0 + tstride * j) * 8 + tl) * (8 * K) + chunk * K;
-        if constexpr (K % 4 == 0)
-        {
-            #pragma unroll
-            for (int i = 0; i < K; i += 4)
-            {
-                uint4 v = *reinterpret_cast<const uint4*>(cp + i);
-                w[j][1 + i] = v.x; w[j][2 + i] = v.y; w[j][3 + i] = v.z; w[j][4 + i] = v.w;
-            }
-        }
-        else if constexpr (K % 2 == 0)
-        {
-            #pragma unroll
-            for (int i = 0; i < K; i += 2)
-            {
-                uint2 v = *reinterpret_cast<const uint2*>(cp + i);
-                w[j][1 + i] = v.x; w[j][2 + i] = v.y;
-            }
-        }
-        else
-        {
-            #pragma unroll
-            for (int i = 0; i < K; ++i) w[j][1 + i] = cp[i];
-        }
-    }
-    #pragma unroll
-    for (int j = 0; j < 4; ++j)
-        w[j][0] = __shfl_sync(0xffffffffu, w[j][K], prev_lane);      // last word of the preceding chunk (cyclic in the tile)
-}
 
 int get_weight_tmap(const void* B, int k, int n, int K, CUtensorMap* out);
 extern unsigned long long* g_tc_dbg;

@@ -318,8 +318,8 @@ def exl3_gemm_allreduce(A, B, C, suh, A_had, svh, mcg, mul1) -> int:
 
 
 # Dense exl3_mgemm calls the int8 tensor-core kernel cannot take (other codebooks, or 5..32 rows: the reference's model code
-# fuses k+v and gate+up up to 32 rows, modules/attn.py:603, modules/mlp.py:726) are issued as one exact tcgen05 exl3_gemm per
-# matrix (tag 200; same results as separate calls, verified against the fused CUDA-core kernels in round 2).  That needs the
+# fuses k+v and gate+up up to 32 rows, modules/attn.py:603, modules/mlp.py:726) are issued as one exact tensor-core exl3_gemm per
+# matrix (tag 200; same results as separate calls, checked against the fused CUDA-core kernels by the tests).  That needs the
 # pointer tables' VALUES on the host, so each table tensor is copied back once and remembered for as long as that tensor
 # object lives and is not modified (weak reference + version counter; never keyed on an address, which the caching allocator
 # reuses).  A table first seen during CUDA-graph capture cannot be copied: such a call runs on the CUDA-core multi-matrix
@@ -541,7 +541,7 @@ def exl3_gemv(A, B, C, suh, A_had, svh, mcg, mul1) -> None:
     Direct entry of the reference's small-m GEMV kernel, exposed for testing (exllamav3_ext/quant/exl3_gemv.cu:171-243,
     bindings.cpp:127): errors if the call is not hard-eligible for that kernel (suh/A_had/svh given, m <= 8, K in 2..4,
     k % 128 == 0, n % 128 == 0; exl3_gemv.cu:36-47,198).  Here small-m calls have no separate kernel family -- the
-    tcgen05 decode-GEMM is the small-m kernel -- so the same eligibility rules are enforced and the call is exl3_gemm.
+    tensor-core decode-GEMM is the small-m kernel -- so the same eligibility rules are enforced and the call is exl3_gemm.
     """
     _need_cuda(A, B, C, suh, A_had, svh)
     if B.dim() != 3:
@@ -568,9 +568,9 @@ def exl3_gemv_int8_max_k(device: int) -> int:
     """
     The reference's model code asks this to decide whether same-input projections (k+v, gate+up) go out as ONE fused
     exl3_mgemm or as separate calls: it unfuses mul1 tensors with K <= this value because its separate int8 GEMVs beat its
-    fused kernel there (model/config.py:48-64 use_mgemm, exllamav3_ext/quant/exl3_gemv_int8.cu:46-52: 6 on Blackwell).
-    Here the fused launch is always the faster one (one launch of the same tensor-core kernel, CTA groups per matrix;
-    profiles/r01_ncu_notes.md item 10), so the answer is 0: use_mgemm() then returns True for every K.
+    fused kernel there (model/config.py:48-64 use_mgemm, exllamav3_ext/quant/exl3_gemv_int8.cu:46-52: 6 on Hopper).
+    Here the fused call is one launch of the same tensor-core kernel with one CTA group per matrix, so the answer is 0:
+    use_mgemm() then returns True for every K.
     """
     _check(_lib.exl3b_num_sms(int(device)))          # same failure mode as the reference on a bad device index
     return 0
@@ -578,7 +578,7 @@ def exl3_gemv_int8_max_k(device: int) -> int:
 
 def exl3_gemm_num_kernel_shapes() -> int:
     """The reference enumerates 4 mma.sync tile shapes (exl3_kernel_map.cuh:53-60) that force_shape_idx selects; here the
-    selectable kernels are 1 = CUDA-core twin, 2 = exact tcgen05 kernel (exl3_gemm honours force_shape_idx 1 / 2 per call);
+    selectable kernels are 1 = CUDA-core twin, 2 = exact tensor-core kernel (exl3_gemm honours force_shape_idx 1 / 2 per call);
     the int8 tensor-core path is what automatic selection (-1) adds for mul1 at <= 4 rows."""
     return 2
 

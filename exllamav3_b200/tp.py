@@ -7,7 +7,7 @@ touches the qgemm path (SURVEY.md 8e):
   * one all-reduce (sum) per row-parallel output, called by the CALLER of the linear (modules/mlp.py:769-770,
     modules/attn.py:546-547) -- here `row_parallel_forward`.
 
-One process per GPU, torch.distributed for the plumbing (backend "nccl" over NVLink on B200 boxes; "gloo" in the CPU
+One process per GPU, torch.distributed for the plumbing (backend "nccl" over NVLink on multi-GPU boxes; "gloo" in the CPU
 tests).  The reference's NCCL backend casts fp32 payloads to bf16 on the wire (model/model_tp_backend.py:119-126);
 we reduce in the tensor's own dtype.
 

@@ -1,8 +1,8 @@
 /*
- * exl3b200 -- Blackwell-native (sm_100a) EXL3 quantized-GEMM path, C ABI.
+ * exl3b200 -- Hopper-native (sm_90a) EXL3 quantized-GEMM path, C ABI.
  *
- * Drop-in boundary for the hot path of turboderp-org/exllamav3 (reference paths are relative to
- * /root/reference/exllamav3/).  Every entry point replaces one pybind11 binding of the reference's
+ * Drop-in boundary for the hot path of turboderp-org/exllamav3 (reference paths are relative to the
+ * exllamav3 package directory of its checkout).  Every entry point replaces one pybind11 binding of the reference's
  * `exllamav3_ext` module; the reference-side shim a maintainer would add is shown in INTEGRATION.md and is
  * implemented in exllamav3_b200/ext.py (ctypes).
  *
@@ -53,8 +53,8 @@ enum exl3b_status
 /* Kernel-path tags returned by exl3b_gemm / exl3b_mgemm */
 #define EXL3B_TAG_NOP 0        /* empty problem                                            */
 #define EXL3B_TAG_SIMT 100     /* CUDA-core bring-up kernel                                */
-#define EXL3B_TAG_TC 200       /* tcgen05 / TMEM decode-GEMM, bit-exact fp16 weights       */
-#define EXL3B_TAG_TC_I8 210    /* tcgen05 kind::i8 codebook path: mul1, m <= 4 (auto); m <= 8 with m*k <= 32768 when forced */
+#define EXL3B_TAG_TC 200       /* wgmma decode-GEMM, bit-exact fp16 weights                */
+#define EXL3B_TAG_TC_I8 210    /* wgmma u8 x s8 codebook path: mul1, m <= 4 (auto); m <= 8 with m*k <= 32768 when forced */
 #define EXL3B_TAG_TC_I8_ROUTED 212 /* routed / weighted exl3b_mgemm (MoE decode) on the kind::i8 kernel: mul1, m <= 4 (auto) */
 #define EXL3B_TAG_TC_I8_CHAIN 220 /* persistent multi-GEMM kernel (exl3b_chain_*; exl3b_gemm when forced): mul1, m <= 4 */
 #define EXL3B_TAG_TC_I8_AR 211 /* the same kernel with the tensor-parallel sum fused into its epilogue (exl3b_gemm_allreduce) */
@@ -77,7 +77,7 @@ int exl3b_set_gemm_path(int tag);
 /*
  * Launch-geometry introspection -- the counterpart of ext.exl3_gemm_num_kernel_shapes / ext.exl3_gemm_shape_compat
  * (exllamav3_ext/bindings.cpp:128-129, exllamav3_ext/quant/exl3_kernel_map.cu:23-75): which kernel path a call takes and with
- * what persistent grid, shared-memory ring and TMEM staging, computed by the same host functions the launchers use.  Pure
+ * what persistent grid and shared-memory ring, computed by the same host functions the launchers use.  Pure
  * host arithmetic: needs no device (num_sms is an argument), so shapes can be vetted without a GPU.
  * exl3b_plan_unit_range / exl3b_plan_cta_of_unit expose the stream-K partition of `units` 128x128 work units (k fastest)
  * over `grid` CTAs: CTA c owns [units*c/grid, units*(c+1)/grid).
@@ -85,12 +85,13 @@ int exl3b_set_gemm_path(int tag);
 struct exl3b_plan
 {
     int32_t path;        /* EXL3B_TAG_*                                                                  */
-    int32_t passes;      /* launches of the GEMM kernel (exact path: ceil(m / 256))                      */
+    int32_t passes;      /* launches of the GEMM kernel (exact path: ceil(m / 128))                      */
     int32_t rows;        /* rows the kernel variant is built for (i8 path: 4 or 8; exact path: m rounded up to 16) */
     int32_t grid;        /* CTAs                                                                         */
     int32_t stages;      /* shared-memory ring depth                                                     */
     int32_t smem_bytes;  /* dynamic shared memory per CTA                                                */
-    int32_t a_stages, d_bufs, tmem_cols;     /* TMEM operand stages / accumulator buffers / columns      */
+    int32_t a_stages, d_bufs, tmem_cols;     /* operand stages / accumulator buffers / tensor-memory columns: on sm_90a
+                                                a_stages = tmem_cols = 0, d_bufs = accumulator hand-off buffers */
     int32_t reserved;
     int64_t units;       /* 128 x 128 work units                                                         */
 };
@@ -111,7 +112,7 @@ int exl3b_plan_cta_of_unit(int64_t units, int grid, int64_t unit);
  *   A_had  (m, k) fp16 scratch for the transformed input; may alias A; may be NULL (library scratch is used)
  *   svh    (n) fp16 or NULL (NULL: no output transform)
  *   k % 128 == 0, n % 128 == 0, 1 <= K <= 8.
- *   force_shape_idx (exl3_gemm.cuh:28): <= 0 automatic; 1 = CUDA-core twin, 2 = exact tcgen05 kernel for THIS call (what
+ *   force_shape_idx (exl3_gemm.cuh:28): <= 0 automatic; 1 = CUDA-core twin, 2 = exact tensor-core kernel for THIS call (what
  *   science/qgemm_benchmark.py uses to time every kernel "shape"); larger values are an error.
  *   force_num_sms (exl3_gemm.cuh:32): > 0 caps the persistent grid.
  */
@@ -153,7 +154,7 @@ int exl3b_mgemm(void* stream,
  * copy once:
  *   exl3b_register_widths(size_n_list (device address, the key), host_widths, count)     count = 0 forgets the entry
  * exl3b_mgemm then runs registered fan-outs (mul1, <= 4 rows, widths multiples of 128, <= 8 matrices, no indices) as ONE
- * launch of the tcgen05 int8 kernel; unregistered lists, or shapes outside that envelope, take the generic path as before.
+ * launch of the wgmma int8 kernel; unregistered lists, or shapes outside that envelope, take the generic path as before.
  * The entry is the caller's promise about the memory at that address: withdraw or renew it when the tensor is rewritten or
  * freed (a recycled address would otherwise inherit the old widths; the shim in ext.py ties the entry to the tensor object and
  * its version counter and withdraws it when the object dies).
@@ -267,7 +268,7 @@ int exl3b_gemm_host(void* stream,
  * launched (the caller falls back to exl3b_gemm + its own all-reduce).  Returns EXL3B_TAG_TC_I8_AR.
  * exl3b_tp_attach_loopback(): single-process bring-up -- "peer" buffers are local allocations, peer partials are supplied
  * with exl3b_tp_debug_inject (tests only).
- * STATUS: verified on one and two B200s in round 2 (tests/test_tp_fused.py).
+ * Tests: tests/test_tp_fused.py (one GPU: loop-back protocol; -m multigpu: two GPUs).
  */
 #define EXL3B_TP_HANDLE_BYTES 64
 int exl3b_tp_alloc(int rank, int world, int64_t max_elems, void* handle_out);

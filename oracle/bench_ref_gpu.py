@@ -1,10 +1,10 @@
 """
 TEST/MEASUREMENT INFRASTRUCTURE.  Times the UNMODIFIED reference kernels (oracle/_ref) and this repo's kernels on the
-same B200, same shapes, same method: per shape, >= 512 MB of rotated weight copies to defeat L2 (as the reference's
-science/qgemm_benchmark.py:74-82), 10 warm-up + 60 timed calls, CUDA events.  "The Blackwell bar" of SURVEY.md 8(d).
+same GPU, same shapes, same method: per shape, >= 512 MB of rotated weight copies to defeat L2 (as the reference's
+science/qgemm_benchmark.py:74-82), 10 warm-up + 60 timed calls, CUDA events.
 
     python oracle/bench_ref_gpu.py [mma|gemv|int8|ours]      (no arg: runs all four in fresh processes)
-    -> gpurun_out/ref_bench_<mode>.json
+    -> $REF_BENCH_OUT/ref_bench_<mode>.json
 """
 import os, sys, json, subprocess
 HERE = os.path.dirname(os.path.abspath(__file__)); ROOT = os.path.dirname(HERE)
@@ -81,7 +81,7 @@ def main(mode):
         print(mode, res[-1], flush=True)
         del Bs
         torch.cuda.empty_cache()
-    out_dir = os.environ.get("REF_BENCH_OUT") or os.path.join(ROOT, "gpurun_out")
+    out_dir = os.environ.get("REF_BENCH_OUT") or os.path.join(ROOT, "ref_bench_out")
     os.makedirs(out_dir, exist_ok=True)
     json.dump(res, open(os.path.join(out_dir, f"ref_bench_{mode}.json"), "w"), indent=1)
 

@@ -1,12 +1,12 @@
 """
-TEST INFRASTRUCTURE (oracle) -- builds oracle/_ref/exl3_ref_ext.so from the UNMODIFIED reference sources
-where they lie under /root/reference (nothing is copied into the repo; outputs go only to oracle/_ref/,
-which is git-ignored but travels to the GPU box).
+TEST INFRASTRUCTURE (oracle) -- builds oracle/_ref/exl3_ref_ext.so from the UNMODIFIED reference sources of the
+exllamav3 checkout at $EXLLAMAV3_SOURCE, by default BASELINE.json's reference_path (nothing is copied into the repo; outputs go only to oracle/_ref/,
+which is git-ignored).
 
 This is our own short recipe (nvcc/g++ on the reference's own source files + oracle/ref_bindings.cpp); the
 reference's build system (setup.py / torch JIT over ~150 TUs) is not run.  Only the EXL3 qgemm-path TUs are
 compiled.  Used for: golden-vector generation on the GPU box (oracle/gen_golden_gpu.py) and the
-"reference kernel on the same B200" timing in profiles/.
+the "reference kernel on the same GPU" timing of bench.py's qgemm section.
 
 usage: python oracle/build_ref.py [-j N]
 """
@@ -15,7 +15,21 @@ import os, sys, subprocess, sysconfig, glob, hashlib
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference/exllamav3/exllamav3_ext"
+
+
+def reference_root():
+    """The exllamav3 checkout the oracle is built from: $EXLLAMAV3_SOURCE, else the reference_path recorded in BASELINE.json."""
+    p = os.environ.get("EXLLAMAV3_SOURCE", "")
+    if not p:
+        try:
+            import json
+            p = json.load(open(os.path.join(HERE, "..", "BASELINE.json")))["reference_path"]
+        except (OSError, ValueError, KeyError):
+            p = ""
+    return p
+
+
+REF = os.path.join(reference_root(), "exllamav3", "exllamav3_ext") if reference_root() else ""
 OUT = os.path.join(HERE, "_ref")
 OBJ = os.path.join(OUT, "obj")
 SO = os.path.join(OUT, "exl3_ref_ext.so")
@@ -42,7 +56,7 @@ def flags():
               "-D_GLIBCXX_USE_CXX11_ABI=" + str(int(torch._C._GLIBCXX_USE_CXX11_ABI)), "-std=c++17"]
     # flags as in the reference's ext.py:92-96 (-lineinfo -O3 --use_fast_math), arch = this box
     nvcc = ["nvcc", "-c", "-O3", "--use_fast_math", "-lineinfo",
-            "-gencode", "arch=compute_100a,code=sm_100a",
+            "-gencode", "arch=compute_90a,code=sm_90a",
             "-Xcudafe", "--diag_suppress=177", "-Xcudafe", "--diag_suppress=20012",
             "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
             "-D__CUDA_NO_HALF_OPERATORS__", "-D__CUDA_NO_HALF_CONVERSIONS__",
@@ -57,12 +71,12 @@ def flags():
 
 
 def obj_name(src):
-    h = hashlib.md5(src.encode()).hexdigest()[:6]
+    h = hashlib.md5((src + " sm_90a").encode()).hexdigest()[:6]        # the target is part of the object's identity
     return os.path.join(OBJ, os.path.basename(src).rsplit(".", 1)[0] + "_" + h + ".o")
 
 
 def build(jobs=8, verbose=True):
-    if not os.path.isdir(REF):
+    if not REF or not os.path.isdir(REF):
         if os.path.exists(SO):
             return SO
         raise RuntimeError("reference sources not present and no prebuilt oracle/_ref")

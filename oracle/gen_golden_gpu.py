@@ -1,11 +1,11 @@
 """
 TEST INFRASTRUCTURE (oracle).  Runs the UNMODIFIED reference CUDA kernels (oracle/_ref/exl3_ref_ext.so, built by
-oracle/build_ref.py from /root/reference) on a B200 and records their outputs on seeded inputs as golden vectors.
+oracle/build_ref.py from $EXLLAMAV3_SOURCE) on a GPU and records their outputs on seeded inputs as golden vectors.
 
     python oracle/gen_golden_gpu.py            # driver: runs the three modes below in fresh processes
-    -> gpurun_out/ref_gpu_mma.npz    EXL3_INT8_GEMV=0 EXL3_GEMV=0   (tensor-core mma.sync kernel only)   == GOLDEN
-       gpurun_out/ref_gpu_gemv.npz   EXL3_INT8_GEMV=0               (fp16-accumulate GEMV heuristics on)
-       gpurun_out/ref_gpu_int8.npz   defaults                       (int8-activation GEMV for mul1, ~0.9% RMS by design)
+    -> $GOLDEN_OUT/ref_gpu_mma.npz    EXL3_INT8_GEMV=0 EXL3_GEMV=0   (tensor-core mma.sync kernel only)   == GOLDEN
+       $GOLDEN_OUT/ref_gpu_gemv.npz   EXL3_INT8_GEMV=0               (fp16-accumulate GEMV heuristics on)
+       $GOLDEN_OUT/ref_gpu_int8.npz   defaults                       (int8-activation GEMV for mul1, ~0.9% RMS by design)
 
 tests/golden/ref_gpu.npz is a copy of ref_gpu_mma.npz (committed).  Inputs are NOT stored: they are regenerated
 from oracle.exl3_oracle.make_synthetic / case_inputs with the same seeds at test time (a checksum of every input is
@@ -136,8 +136,9 @@ def main_mode(mode):
         out[f"mgemm_d_{int(fp32)}"] = C[0].cpu().numpy()
     torch.cuda.synchronize()
 
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    path = os.path.join(ROOT, "gpurun_out", f"ref_gpu_{mode}.npz")
+    out_dir = os.environ.get("GOLDEN_OUT") or os.path.join(ROOT, "golden_out")
+    os.makedirs(out_dir, exist_ok=True)
+    path = os.path.join(out_dir, f"ref_gpu_{mode}.npz")
     np.savez_compressed(path, **out)
     print("wrote", path, len(out), "arrays")
 

@@ -1,6 +1,6 @@
 """
 TEST INFRASTRUCTURE (oracle).  Generates tests/golden/ref_py.npz by IMPORTING the reference's own Python helpers
-from /root/reference (this container only; the fixture travels, the reference does not):
+from the exllamav3 checkout of oracle/build_ref.py's reference_root() (the fixture is committed, the reference is not needed by the tests):
 
   * tensor_core_perm                      modules/quant/exl3_lib/quantize.py:22-44
   * get_hadamard(128) (Sylvester)         util/hadamard.py:107-131
@@ -16,7 +16,9 @@ import sys, types, os
 import numpy as np
 import torch
 
-REF = "/root/reference"
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from build_ref import reference_root
+REF = reference_root()
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden", "ref_py.npz")
 
 

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE (oracle) -- not product code.
 //
 // pybind11 stub that exposes the hot-path subset of the UNMODIFIED reference extension
-// (/root/reference/exllamav3/exllamav3_ext, compiled in place by oracle/build_ref.py into oracle/_ref/).
+// (exllamav3/exllamav3_ext of the checkout named by $EXLLAMAV3_SOURCE, compiled in place by oracle/build_ref.py into oracle/_ref/).
 // It only declares/binds functions; all implementations come from the reference's own translation units.
 // The reference's bindings.cpp binds its whole ~150-TU extension; this binds what the EXL3 qgemm path needs
 // (reference bindings: exllamav3_ext/bindings.cpp:118-147).

@@ -7,8 +7,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
-    config.addinivalue_line("markers", "multigpu: needs two or more CUDA devices on one box; run with -m multigpu under gpurun --gpus N")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
+    config.addinivalue_line("markers", "multigpu: needs two or more CUDA devices on one box; run with -m multigpu")
 
 
 def pytest_collection_modifyitems(config, items):

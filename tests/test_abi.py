@@ -153,7 +153,7 @@ def test_mgemm_split_host_logic(monkeypatch):
 
 
 def test_force_shape_idx_validation_without_gpu():
-    """force_shape_idx selects the kernel per call like the reference's (1 = CUDA-core twin, 2 = exact tcgen05); an index
+    """force_shape_idx selects the kernel per call like the reference's (1 = CUDA-core twin, 2 = exact tensor-core kernel); an index
     beyond exl3_gemm_num_kernel_shapes() is an argument error raised before any CUDA work."""
     from exllamav3_b200 import ext
     one = ctypes.c_void_p(16)

@@ -148,12 +148,3 @@ def test_qgemm_section_control_flow(monkeypatch):
     assert {(c[1], c[2]) for c in pre} == {((65536, 256), 256), ((16384, 256), 512)} and len(pre) == 2 * 7
     for v in out["prefill_tensor"].values():
         assert v["tflops"] > 0 and v["frac_of_measured_bf16_burst"] > 0 and v["rows"] in (65536, 16384)
-
-
-def test_ncu_capture_parser_is_unit_aware(tmp_path):
-    # the committed capture: 29.485056 Mbyte read, 0 byte written, for 29.46 MB of algorithmic bytes (no re-reads)
-    b = bench.ncu_dram_bytes(os.path.join(ROOT, bench.NCU_CAPTURE))
-    assert 29.4e6 < b < 29.6e6 and abs(b / bench.alg_bytes(1, 4096, 14336, 4, True) - 1.0) < 2e-3
-    f = tmp_path / "cap.csv"
-    f.write_text("metric,unit,value\ndram__bytes_read.sum,Gbyte,1.5\ndram__bytes_write.sum,Kbyte,2\n")
-    assert bench.ncu_dram_bytes(str(f)) == 1.5e9 + 2e3

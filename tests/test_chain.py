@@ -5,7 +5,7 @@ exl3_gemm(down)) and of BC_Attention's projections (libtorch/attention.cpp:286-3
 
 CPU part: the kernel's own unit cursor replayed on the host (every unit of every stage visited exactly once over the grid, run
 and accumulation-chunk bounds, quad ownership), launch geometry, argument validation.
-GPU part: parity with the fp64 oracle (tolerances of DESIGN.md 5: max-abs <= 2e-3 max|y|, rel-RMS <= 1e-3) and with separate
+GPU part: parity with the fp64 oracle (tolerances of README.md, Parity: max-abs <= 2e-3 max|y|, rel-RMS <= 1e-3) and with separate
 exl3_gemm calls, for single ops (every K, 1..4 rows, fp16 / fp32 outputs), same-input stages, dependent stages with the
 gated activation in between, at test sizes and at the Llama shapes.
 """

@@ -129,7 +129,7 @@ def test_emulation_builds_from_the_library_header():
 def test_i8_path_arithmetic_from_device_headers_matches_oracle_model(emu, K):
     """
     The int8 tensor-core path's arithmetic, run on the host FROM THE DEVICE HEADERS (csrc/i8_math.cuh digits + reassembly,
-    csrc/decode.cuh product words, byte sums standing in for tcgen05.mma.kind::i8), against the oracle's independent fp64
+    csrc/decode.cuh product words, byte sums standing in for the u8 x s8 wgmma), against the oracle's independent fp64
     model of the path (oracle.exl3_gemm_i8_model): same result to fp32 round-off.  Also asserts what the kernel relies on:
     digits replicated over four bytes, hi in [-127, 127], s32 accumulators never overflow at these sizes.
     """

@@ -1,7 +1,7 @@
 """
 Fan-out launches: exl3_mgemm with per-matrix output widths (size_n_list / c_ptrs; exllamav3_ext/quant/exl3_gemm.cu:402-447,
 exl3_gemm_kernel.cuh:172-181; used by the reference for same-input projections, libtorch/dsv4_attn.cpp:88-99) as ONE launch of the
-tcgen05 int8 kernel.  CPU: the CTA-group partition and the width registry.  GPU: parity of the fused call with the separate calls
+wgmma int8 kernel.  CPU: the CTA-group partition and the width registry.  GPU: parity of the fused call with the separate calls
 and with the oracle on the Llama q + k + v shapes (8B, and a 70B TP-8 shard), shared and per-matrix inputs, graph replay, fall-backs.
 """
 import numpy as np

@@ -3,11 +3,11 @@ Full-size parity of the DEFAULT product path (automatic kernel selection, throug
 closing the holes the round-1 review listed: lm_head 4096 x 128256 at 6 bpw, the Llama-3.1-8B shapes at 2 / 3 / 6 bpw (config 3),
 8 and 32 rows at full size, every Llama-3.1-70B shard shape at TP 2 / 4 / 8 including k = 28672 (224 k-blocks: beyond the
 96-unit int32 accumulation chunk), dense multi-matrix calls at 8 / 32 rows, per-matrix output widths (size_n_list / c_ptrs), and
-the dense tcgen05 GEMM at 8192 x 4096 x 14336.
+the dense wgmma GEMM at 8192 x 4096 x 14336.
 
 Method at sizes the fp64 oracle cannot afford in full: random 128-column blocks of the output against the oracle restricted to
 those columns (a 128-column block of an EXL3 linear is itself a complete EXL3 linear: trellis[:, 8b:8b+8], svh[128b:128b+128]),
-tolerances of DESIGN.md 5 (max-abs <= 2e-3 max|y| (+1 fp16 ulp), rel-RMS <= 1e-3).
+tolerances of README.md, Parity (max-abs <= 2e-3 max|y| (+1 fp16 ulp), rel-RMS <= 1e-3).
 """
 import numpy as np
 import pytest
@@ -82,7 +82,7 @@ def test_llama_shapes_other_bitrates(cuda, K, shape):
     x = torch.from_numpy(rng.standard_normal((1, k)).astype(np.float16)).to(cuda)
     y, _ = run_default(ext, x, tr, suh, svh, True)
     check_blocks(y, x.cpu().numpy(), tr, suh, svh, K, 2, rng.choice(n // 128, 3, replace=False), tag=f"{shape} K={K}")
-    # the other codebooks take the exact tcgen05 kernel at one row: same bar
+    # the other codebooks take the exact tensor-core kernel at one row: same bar
     for (mcg, cb) in ((False, 0), (True, 1)):
         y, tag = run_default(ext, x, tr, suh, svh, True, mul1=False, mcg=mcg)
         assert tag == ext.EXL3B_TAG_TC
@@ -184,7 +184,7 @@ def test_mgemm_per_matrix_widths(cuda, m):
 
 
 def test_hgemm_prefill_size(cuda):
-    """Dense tcgen05 GEMM at a prefill shape (8192 x 4096 x 14336, the largest of profiles/r01_hgemm_tcgen05_vs_cublas.jsonl):
+    """Dense wgmma GEMM at a prefill shape (8192 x 4096 x 14336):
     sampled rows / columns against an fp64 dot product of the same fp16 operands."""
     from exllamav3_b200 import ext
     m, k, n = 8192, 4096, 14336

@@ -1,5 +1,5 @@
 """
-GPU parity tests (B200): the CUDA path, called through the C ABI (exllamav3_b200.ext -> libexl3b200.so), against the
+GPU parity tests (H100): the CUDA path, called through the C ABI (exllamav3_b200.ext -> libexl3b200.so), against the
 CPU oracle on the same seeded inputs, against the committed golden outputs of the reference's own CUDA kernels, and
 -- at BASELINE.json's full sizes -- through size-independent properties.
 
@@ -95,7 +95,7 @@ def test_had_r_128_bitexact(cuda, dt, mode):
 
 @pytest.fixture(params=["tc", "simt"])
 def gemm_path(request):
-    """Run the test once per kernel path: tcgen05 (default product path) and the CUDA-core path."""
+    """Run the test once per kernel path: tensor cores (default product path) and the CUDA-core path."""
     from exllamav3_b200 import ext
     prev = ext.set_gemm_path(ext.EXL3B_TAG_TC if request.param == "tc" else ext.EXL3B_TAG_SIMT)
     yield request.param
@@ -113,7 +113,7 @@ def test_gemm_vs_oracle(cuda, gemm_path, K, cb, m):
         y, xh, tag = run_gemm(ext, cuda, x, tr, suh, svh, K, cb, fp32)
         assert tag == (ext.EXL3B_TAG_TC if gemm_path == "tc" else ext.EXL3B_TAG_SIMT)
         assert not np.isnan(y.astype(np.float32)).any()
-        if gemm_path == "simt":      # the tcgen05 path keeps its transformed input in a private tiled buffer
+        if gemm_path == "simt":      # the tensor-core path keeps its transformed input in a private tiled buffer
             xh_ref = orc.had_r_128(x, pre_scale=suh)
             assert (xh.view(np.uint16) == xh_ref.view(np.uint16)).all()      # input transform bit-exact
         mx, rms = rel_err(y, ref)
@@ -178,14 +178,14 @@ def test_reconstruct_had(cuda, K, cb):
 
 @pytest.mark.parametrize("K,cb", [(1, 0), (2, 1), (3, 2), (4, 2), (5, 0), (6, 2), (7, 1), (8, 2)])
 def test_reconstruct_had_tensor_core_and_cuda_core_twins(cuda, K, cb):
-    # reconstruct_tc.cu (both Hadamards as tcgen05 GEMMs, the default) against the oracle and against the CUDA-core
+    # reconstruct_tc.cu (both Hadamards as wgmma GEMMs, the default) against the oracle and against the CUDA-core
     # kernel of kernels_basic.cu on a shape with more blocks than one wave of the persistent grid covers per CTA
     from exllamav3_b200 import ext
     k, n = 1024, 5120 if K <= 4 else 2560
     tr, suh, svh, _ = orc.make_synthetic(k, n, K, seed=K * 10 + cb)
     outs = {}
     try:
-        for mode in (1, 2, 21, 22, 24):              # CUDA cores; tensor cores: default, 1 / 2 / 4 threads per row
+        for mode in (1, 2):                          # CUDA cores, tensor cores
             ext.lib.exl3b_debug_reconstruct_had(mode)
             w = torch.full((k, n), float("nan"), dtype=torch.half, device=cuda)
             ext.reconstruct_had_slice(w, T(tr, cuda), T(suh, cuda), T(svh, cuda), K, cb == 1, cb == 2, 0)
@@ -201,8 +201,6 @@ def test_reconstruct_had_tensor_core_and_cuda_core_twins(cuda, K, cb):
     for mode in outs:
         assert np.isfinite(outs[mode]).all()
         assert np.abs(outs[mode][:256] - ref).max() / np.abs(ref).max() < 2e-3, mode
-    for mode in (21, 22, 24):
-        assert np.array_equal(outs[mode], outs[2]), mode        # the thread split does not change a single bit
     # the two kernels round at the same places (fp16 tile between the passes, fp16 scale multiplies): they differ by
     # the summation order inside the 128-term sums only, i.e. by a few fp16 ulps on few elements
     d = np.abs(outs[1] - outs[2])
@@ -256,32 +254,26 @@ def test_hgemm(cuda):
     assert rel_err(cfull[:, 128:256].cpu().numpy(), ref)[0] <= 2e-3 and float(cfull[:, :128].abs().max()) == 0.0
 
 
-@pytest.mark.parametrize("mode", [1, 2])
-def test_hgemm_single_cta_and_cta_pair_tiles(cuda, mode):
-    """Both tile modes of the dense tcgen05 GEMM on the same inputs: 1 = one CTA per 128 x 256 tile, 2 = a CTA pair
-    (tcgen05.mma.cta_group::2) per 256 x 256 tile -- ragged m / n / k, a single 128-row tile (second CTA of the pair all out of
-    range), strided C, both output types; against an fp64 product of the fp16 operands (the reference's hgemm is cuBLAS, hgemm.cu:19-102)."""
+def test_hgemm_tensor_core_tiles(cuda):
+    """The dense wgmma GEMM (128 x 128 tiles, persistent CTAs) -- ragged m / n / k, a single tile, several tiles per CTA, strided C,
+    both output types; against an fp64 product of the fp16 operands (the reference's hgemm is cuBLAS, hgemm.cu:19-102)."""
     from exllamav3_b200 import ext
-    rng = np.random.default_rng(mode)
-    ext.lib.exl3b_debug_hgemm_pair(mode)
-    try:
-        for (m, k, n) in ((300, 512, 256), (129, 72, 264), (1, 128, 128), (513, 200, 520), (1024, 1024, 768)):
-            a = rng.standard_normal((m, k)).astype(np.float16); b = rng.standard_normal((k, n)).astype(np.float16)
-            ref = a.astype(np.float64) @ b.astype(np.float64)
-            for dt in (torch.half, torch.float):
-                c = torch.full((m, n), float("nan"), dtype=dt, device=cuda)
-                ext.hgemm(T(a, cuda), T(b, cuda), c)
-                torch.cuda.synchronize()
-                assert not torch.isnan(c.float()).any(), (mode, m, k, n, dt)
-                mx, rms = rel_err(c.cpu().numpy(), ref)
-                assert mx <= (2e-3 if dt == torch.half else 1e-4), (mode, m, k, n, dt, mx)
-        a = rng.standard_normal((260, 128)).astype(np.float16); b = rng.standard_normal((128, 128)).astype(np.float16)
-        cfull = torch.zeros((260, 384), dtype=torch.half, device=cuda)
-        ext.hgemm(T(a, cuda), T(b, cuda), cfull[:, 128:256])
-        assert rel_err(cfull[:, 128:256].cpu().numpy(), a.astype(np.float64) @ b.astype(np.float64))[0] <= 2e-3
-        assert float(cfull[:, :128].abs().max()) == 0.0 and float(cfull[:, 256:].abs().max()) == 0.0
-    finally:
-        ext.lib.exl3b_debug_hgemm_pair(0)
+    rng = np.random.default_rng(1)
+    for (m, k, n) in ((300, 512, 256), (129, 72, 264), (1, 128, 128), (513, 200, 520), (1024, 1024, 768), (4096, 256, 4352)):
+        a = rng.standard_normal((m, k)).astype(np.float16); b = rng.standard_normal((k, n)).astype(np.float16)
+        ref = a.astype(np.float64) @ b.astype(np.float64)
+        for dt in (torch.half, torch.float):
+            c = torch.full((m, n), float("nan"), dtype=dt, device=cuda)
+            ext.hgemm(T(a, cuda), T(b, cuda), c)
+            torch.cuda.synchronize()
+            assert not torch.isnan(c.float()).any(), (m, k, n, dt)
+            mx, rms = rel_err(c.cpu().numpy(), ref)
+            assert mx <= (2e-3 if dt == torch.half else 1e-4), (m, k, n, dt, mx)
+    a = rng.standard_normal((260, 128)).astype(np.float16); b = rng.standard_normal((128, 128)).astype(np.float16)
+    cfull = torch.zeros((260, 384), dtype=torch.half, device=cuda)
+    ext.hgemm(T(a, cuda), T(b, cuda), cfull[:, 128:256])
+    assert rel_err(cfull[:, 128:256].cpu().numpy(), a.astype(np.float64) @ b.astype(np.float64))[0] <= 2e-3
+    assert float(cfull[:, :128].abs().max()) == 0.0 and float(cfull[:, 256:].abs().max()) == 0.0
 
 
 def test_linear_exl3_kernel_vs_reconstruct_path(cuda):

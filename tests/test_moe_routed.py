@@ -1,11 +1,10 @@
 """
-Routed / weighted exl3_mgemm (the reference's MoE decode calls, modules/block_sparse_mlp.py:1362-1421) on the tcgen05 int8
+Routed / weighted exl3_mgemm (the reference's MoE decode calls, modules/block_sparse_mlp.py:1362-1421) on the wgmma int8
 path (csrc/gemm_tc_i8_routed.cu, tag 212), against the CPU oracle's restatement of the mgemm semantics
 (exllamav3_ext/quant/exl3_gemm.cu:341-381) and against the verified default path (CUDA-core kernels, tag 100) on the same
 inputs.
 
-Verified on a B200 in round 2 (gpurun_out/r02_call1); routed mul1 calls at <= 4 rows take this path automatically, the tests
-also force it explicitly and compare with the CUDA-core twin (EXL3B_TAG_SIMT).
+Routed mul1 calls at <= 4 rows take this path automatically; the tests also force it explicitly and compare with the CUDA-core twin (EXL3B_TAG_SIMT).
 """
 import os
 import numpy as np
@@ -142,7 +141,7 @@ def test_routed_i8_mgemm_mixtral_shapes_properties(cuda):
 @pytest.mark.gpu
 @pytest.mark.parametrize("m,cb", [(8, 2), (32, 2), (1, 0), (17, 1)])
 def test_mgemm_split_matches_fused_default(cuda, monkeypatch, m, cb):
-    """EXL3B_MGEMM_SPLIT (ext.py): dense multi-matrix calls the int8 kernel cannot take, issued as one exact tcgen05 exl3_gemm
+    """EXL3B_MGEMM_SPLIT (ext.py): dense multi-matrix calls the int8 kernel cannot take, issued as one exact tensor-core exl3_gemm
     per matrix, against the default (CUDA-core multi-matrix kernels) and the fp64 oracle."""
     from exllamav3_b200 import ext
     k, n, K, nm = 512, 384, 4, 2

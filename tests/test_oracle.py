@@ -2,7 +2,7 @@
 Oracle self-checks and pinning (CPU only).  The oracle (oracle/exl3_oracle.py) is the checker for the CUDA path;
 these tests pin the checker itself:
   * fixtures produced by importing the reference's own Python helpers (tests/golden/ref_py.npz, oracle/gen_golden_py.py)
-  * outputs of the reference's own CUDA kernels captured on a B200 (tests/golden/ref_gpu.npz, oracle/gen_golden_gpu.py)
+  * outputs of the reference's own CUDA kernels (tests/golden/ref_gpu.npz, oracle/gen_golden_gpu.py)
   * format invariants the reference's tests assert (tests/test_quant_fn.py:82-87,100-128)
   * the C restatement (oracle/exl3_oracle.c) against the numpy one
 """
@@ -154,7 +154,7 @@ def test_c_oracle_matches_numpy(K, cb):
     assert (out.view(np.uint16) == orc.reconstruct(tr, K, cb).view(np.uint16)).all()
 
 
-# ---- pinned against the reference's CUDA kernels (captured on B200) ------------------------------------------------
+# ---- pinned against the reference's CUDA kernels (captured outputs) ------------------------------------------------
 
 def _gpu_golden():
     p = os.path.join(GOLDEN, "ref_gpu.npz")
@@ -176,7 +176,7 @@ RECHAD_CASES = [(4, 2, 128, 384, 128, 256), (3, 0, 128, 256, 0, 256)]        # o
 
 
 def test_reconstruct_had_vs_reference_cuda_golden():
-    """The fused reconstruction as the reference's OWN kernel computed it on a B200: the fp64 restatement reproduces it within the
+    """The fused reconstruction as the reference's OWN kernel computed it: the fp64 restatement reproduces it within the
     reference's test bound (its kernel adds in fp16), and the fp32-sum model the CUDA kernels of this repo follow is closer to fp64
     than the reference's output is."""
     g = _gpu_golden()

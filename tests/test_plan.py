@@ -1,6 +1,6 @@
 """
-Host logic of the tcgen05 launchers, checked WITHOUT a GPU through exl3b_gemm_plan / exl3b_plan_* (the same functions the
-launchers call): path selection, shared-memory / TMEM / workspace budgets and the persistent stream-K partition, for every
+Host logic of the tensor-core launchers, checked WITHOUT a GPU through exl3b_gemm_plan / exl3b_plan_* (the same functions the
+launchers call): path selection, shared-memory / workspace budgets and the persistent stream-K partition, for every
 shape of BASELINE.json's configs -- Llama-3.1-8B and 70B, their tensor-parallel shards at 2/4/8 ranks (SURVEY.md 8d) and
 the Mixtral expert shapes -- and every bitrate, i.e. also for shapes no GPU test runs at full size.
 
@@ -14,7 +14,7 @@ The partition invariants are what the kernels' split-K combine relies on (gemm_t
 import ctypes
 import pytest
 
-SMS = 148
+SMS = 132
 TAG_SIMT, TAG_TC, TAG_I8 = 100, 200, 210
 
 
@@ -59,14 +59,14 @@ def model_shapes():
 
 
 def test_path_selection_rules(lib):
-    # mul1 at m <= 4 -> int8 tensor-core path; everything else the exact tcgen05 path (api.cu select_gemm_path)
+    # mul1 at m <= 4 -> int8 tensor-core path; everything else the exact tensor-core path (api.cu select_gemm_path)
     assert plan(lib, 1, 4096, 4096, 4, 2).path == TAG_I8
     assert plan(lib, 4, 4096, 4096, 4, 2).path == TAG_I8
     assert plan(lib, 5, 4096, 4096, 4, 2).path == TAG_TC
     assert plan(lib, 1, 4096, 4096, 4, 0).path == TAG_TC
     assert plan(lib, 1, 4096, 4096, 4, 1).path == TAG_TC
     p = plan(lib, 1000, 4096, 4096, 4, 2)
-    assert p.path == TAG_TC and p.passes == 4 and p.rows == 256
+    assert p.path == TAG_TC and p.passes == 8 and p.rows == 128
     # forced paths (exl3b_set_gemm_path), including the refusal when the forced path cannot take the call
     from exllamav3_b200 import ext
     try:
@@ -87,13 +87,14 @@ def test_path_selection_rules(lib):
 
 
 def test_known_geometry_of_the_bench_shapes(lib):
-    """The launch geometry the round-1 profiles were taken with (profiles/r01_ncu_notes.md): K = 4, m = 1."""
+    """The launch geometry of the bench's decode shapes: K = 4, m = 1."""
     p = plan(lib, 1, 4096, 4096, 4, 2)
-    # stage = 8192 B weights + 4096 + 64 B digits; activation cache 8192 B -> (204800 - 8192) // 12352 = 15 stages
-    assert (p.rows, p.grid, p.units, p.stages, p.a_stages, p.d_bufs, p.tmem_cols) == (4, 148, 1024, 15, 3, 2, 512)
-    assert p.smem_bytes == 15 * 12352 + 16 * 128 * 4 + 1024 + 8192
+    # stage = 8192 B weights + 4096 + 64 B digits; accumulator hand-off 16512 B; activation cache 8192 B
+    # -> (204800 - 16512 - 8192) // 12352 = 14 stages; no tensor memory on sm_90a (accumulators in registers)
+    assert (p.rows, p.grid, p.units, p.stages, p.a_stages, p.d_bufs, p.tmem_cols) == (4, 132, 1024, 14, 0, 2, 0)
+    assert p.smem_bytes == 14 * 12352 + 16 * 128 * 4 + 1024 + 16512 + 8192
     p = plan(lib, 1, 4096, 128256 // 128 * 128, 6, 2)          # lm_head, 6 bpw
-    assert p.grid == 148 and p.units == 32 * 1002 and p.stages == (204800 - 8192) // (12288 + 4160)
+    assert p.grid == 132 and p.units == 32 * 1002 and p.stages == (204800 - 16512 - 8192) // (12288 + 4160)
     p = plan(lib, 1, 128, 128, 4, 2)                            # a single unit: one CTA
     assert p.grid == 1 and p.units == 1
     p = plan(lib, 1, 4096, 4096, 4, 2, force=64)                # force_num_sms caps the persistent grid
@@ -110,11 +111,12 @@ def test_budgets_for_every_model_shape(lib, K):
             assert p.smem_bytes <= 220 * 1024                   # cudaFuncAttributeMaxDynamicSharedMemorySize set by the launchers
             assert 1 <= p.grid <= min(SMS, p.units) and p.units == (k // 128) * (n // 128)
             assert n // 128 <= 32768                            # DevCtx::COUNTERS_PER_SLOT
+            assert (p.a_stages, p.tmem_cols) == (0, 0)         # no tensor memory on sm_90a
             if p.path == TAG_I8:
                 assert p.grid <= 256                            # DevCtx::I8_PART_CTAS exchange slots
-                assert p.a_stages * 128 + p.d_bufs * 16 <= p.tmem_cols
+                assert p.d_bufs == 2                            # two shared-memory accumulator hand-off buffers
             else:
-                assert p.a_stages * 64 + p.d_bufs * p.rows <= p.tmem_cols
+                assert p.rows <= 128                            # fp32 accumulators of one pass live in registers
                 assert 2 * p.grid * p.rows * 128 * 4 <= 40 << 20   # DevCtx::WS_BYTES_PER_SLOT
 
 

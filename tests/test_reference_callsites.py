@@ -1,70 +1,44 @@
 """
-Drop-in check at the Python level, run where the reference checkout exists (this container; skipped on the GPU box): the
-REFERENCE'S OWN `exllamav3/modules/quant/exl3.py` (LinearEXL3) is loaded from /root/reference -- unmodified, never copied --
-with its `ext` import bound to this repo's shim (`exllamav3_b200.ext`), exactly what INTEGRATION.md's three-line patch does.
-Every call the reference module then makes into the extension is bound against the shim's real signatures (a wrong argument
-count or a missing name fails here), and the reference's dispatch is compared with this repo's own minimal caller (QLinear)
-on the same inputs: both must issue the same extension calls with the same argument shapes.  No kernel runs: the shim's entry points are wrapped by recorders after their signatures have been checked.
+Drop-in check at the Python level against what the REFERENCE'S OWN Python modules do, recorded once by
+oracle/gen_golden_callsites.py into tests/golden/ref_callsites.json.gz: the reference's LinearEXL3 (modules/quant/exl3.py), run
+with its `ext` import bound to this repo's shim (`exllamav3_b200.ext`, exactly what INTEGRATION.md's patch does), issued the
+recorded extension calls; its MultiLinear built the recorded pointer tables; its use_mgemm policy gave the recorded answers;
+its tp_import_split built the recorded shards; and its Python tree calls the qgemm surface at the recorded call sites.  Here
+this repo's own caller (QLinear, pointer_tables, tp.tp_slice) must do the same on the same inputs, and every recorded call
+must bind against the shim's real signatures.  No kernel runs: the shim's entry points are wrapped by recorders.
 """
-import importlib.util, inspect, os, sys, types
+import gzip, inspect, json, os
 import pytest
 import torch
 
-REF = "/root/reference/exllamav3"
-pytestmark = pytest.mark.skipif(not os.path.isfile(os.path.join(REF, "modules", "quant", "exl3.py")),
-                                reason="reference checkout not present (GPU box)")
+import refstubs
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_callsites.json.gz")
+
+
+@pytest.fixture(scope="module")
+def gold():
+    with gzip.open(GOLDEN, "rt") as f:
+        return json.load(f)
 
 
 @pytest.fixture()
-def ref_exl3(monkeypatch):
+def recorder(monkeypatch):
     from exllamav3_b200 import ext
-    import refstubs
     calls = []
 
     def wrap(name):
-        real = getattr(ext, name)
-        sig = inspect.signature(real)
+        sig = inspect.signature(getattr(ext, name))
 
         def f(*a, **kw):
-            sig.bind(*a, **kw)                                    # the reference's argument list fits the shim's signature
-            calls.append((name,) + tuple(tuple(t.shape) if isinstance(t, torch.Tensor) else t for t in a))
+            sig.bind(*a, **kw)
+            calls.append([name, [refstubs.encode(t) for t in a], sorted(kw)])
             return 210
         return f
 
-    for name in ("exl3_gemm", "had_r_128", "reconstruct", "reconstruct_slice", "reconstruct_had_slice", "hgemm"):
+    for name in refstubs.RECORDED_OPS:
         monkeypatch.setattr(ext, name, wrap(name))
-
-    def mod(name, **attrs):
-        m = types.ModuleType(name)
-        m.__path__ = []
-        for k, v in attrs.items():
-            setattr(m, k, v)
-        monkeypatch.setitem(sys.modules, name, m)
-        return m
-
-    class Config: pass
-    mod("exllamav3")
-    mod("exllamav3.model")
-    mod("exllamav3.model.config", Config=Config, NullConfig=refstubs.NullConfig)
-    mod("exllamav3.ext", exllamav3_ext=ext)                       # <- INTEGRATION.md: the extension module IS the shim
-    mod("exllamav3.util", profile_opt=lambda f: f)
-    mod("exllamav3.util.tensor", g_tensor_cache=refstubs.g_tensor_cache)
-    mod("exllamav3.modules")
-    mod("exllamav3.modules.quant")
-    mod("exllamav3.modules.quant.exl3_lib")
-    mod("exllamav3.modules.quant.exl3_lib.quantize", preapply_had_l=refstubs.preapply_had_l, preapply_had_r=refstubs.preapply_had_r,
-        had_k=128, had_n=128)
-    spec = importlib.util.spec_from_file_location("exllamav3.modules.quant.exl3", os.path.join(REF, "modules", "quant", "exl3.py"))
-    m = importlib.util.module_from_spec(spec)
-    monkeypatch.setitem(sys.modules, "exllamav3.modules.quant.exl3", m)
-    spec.loader.exec_module(m)
-    return m, calls
-
-
-def _tensors(k, n, K=4):
-    g = torch.Generator().manual_seed(1)
-    tr = torch.randint(0, 32767, (k // 16, n // 16, 16 * K), generator=g, dtype=torch.int32).to(torch.int16)
-    return dict(suh=torch.ones(k, dtype=torch.half), svh=torch.ones(n, dtype=torch.half), trellis=tr, mul1=torch.zeros((), dtype=torch.int))
+    return calls
 
 
 def _qlin(t, **kw):
@@ -72,170 +46,105 @@ def _qlin(t, **kw):
     return QLinear(t["trellis"], t["suh"], t["svh"], mul1=True, **kw)
 
 
-def test_reference_linear_exl3_runs_on_the_shim_and_matches_the_mirror(ref_exl3):
-    ref_mod, calls = ref_exl3
-    from exllamav3_b200 import qlinear
-    assert ref_mod.AUTO_RECONSTRUCT_THRESHOLD == qlinear.KERNEL_MAX_ROWS == 144
-    assert ref_mod.MAX_RECONSTRUCT_SLICE_N == qlinear.DENSE_WINDOW_COLS == 32768
-    k, n = 256, 384
-    ref_lin = ref_mod.LinearEXL3(None, k, n, key="q", **_tensors(k, n))          # constructs ext.BC_LinearEXL3 from the shim
-    mir_lin = _qlin(_tensors(k, n))
+def _binds(call):
     from exllamav3_b200 import ext
-    assert isinstance(ref_lin.bc, ext.BC_LinearEXL3) and ref_lin.K == 4 and ref_lin.mul1 and not ref_lin.mcg
-    for (shape, params, out_dtype) in (((1, k), {}, None), ((144, k), {}, torch.float), ((3, 7, k), {}, None),
-                                       ((145, k), {}, None), ((1, k), {"reconstruct": True}, None), ((1024, k), {}, torch.float)):
-        x = torch.zeros(shape, dtype=torch.half)
-        calls.clear(); yr = ref_lin.forward(x, params, out_dtype); seq_ref = list(calls)
-        calls.clear(); ym = mir_lin.forward(x, params, out_dtype); seq_mir = list(calls)
-        assert seq_ref == seq_mir and len(seq_ref) >= 1, (shape, params)            # same extension calls, same argument shapes
-        assert yr.shape == ym.shape == tuple(shape[:-1]) + (n,) and yr.dtype == ym.dtype
+    name, args, kws = call
+    inspect.signature(getattr(ext, name)).bind(*([None] * len(args)), **{k: None for k in kws})
+
+
+def test_reference_linear_exl3_runs_on_the_shim_and_matches_the_mirror(gold, recorder):
+    from exllamav3_b200 import qlinear, ext
+    g = gold["linear"]
+    assert g["AUTO_RECONSTRUCT_THRESHOLD"] == qlinear.KERNEL_MAX_ROWS == 144
+    assert g["MAX_RECONSTRUCT_SLICE_N"] == qlinear.DENSE_WINDOW_COLS == 32768
+    assert g["bc_type"] == ext.BC_LinearEXL3.__name__ and (g["K"], g["mcg"], g["mul1"]) == (4, False, True)
+    k, n = 256, 384
+    mir = _qlin(refstubs.tensors(k, n))
+    assert len(g["cases"]) == len(refstubs.LINEAR_CASES)
+    for (shape, params, odt), case in zip(refstubs.LINEAR_CASES, g["cases"]):
+        recorder.clear()
+        y = mir.forward(torch.zeros(shape, dtype=torch.half), params, getattr(torch, odt) if odt else None)
+        assert recorder == case["calls"] and len(case["calls"]) >= 1, (shape, params)     # same calls, same argument shapes
+        assert list(y.shape) == case["y_shape"] and str(y.dtype) == case["y_dtype"], (shape, params)
+        for c in case["calls"]:
+            _binds(c)
     # the kernel path hands exl3_gemm the reference's 10 arguments: (A, B, C, suh, A_had, svh, -1, mcg, mul1, 0)
-    calls.clear(); ref_lin.forward(torch.zeros((2, k), dtype=torch.half), {})
-    assert calls[0][0] == "exl3_gemm" and calls[0][7:] == (-1, False, True, 0)
+    last = g["cases"][-1]["calls"][0]
+    assert last[0] == "exl3_gemm" and last[1][6:] == [-1, False, True, 0]
 
 
-def test_reference_wide_output_slicing_matches_the_mirror(ref_exl3, monkeypatch):
-    ref_mod, calls = ref_exl3
+def test_reference_wide_output_slicing_matches_the_mirror(gold, recorder, monkeypatch):
     from exllamav3_b200 import qlinear
-    monkeypatch.setattr(ref_mod, "MAX_RECONSTRUCT_SLICE_N", 256)
     monkeypatch.setattr(qlinear, "DENSE_WINDOW_COLS", 256)
     k, n = 128, 640
-    ref_lin = ref_mod.LinearEXL3(None, k, n, **_tensors(k, n)); mir_lin = _qlin(_tensors(k, n))
-    for rows in (200, 2048):
-        x = torch.zeros((rows, k), dtype=torch.half)
-        calls.clear(); ref_lin.forward(x, {}); a = list(calls)
-        calls.clear(); mir_lin.forward(x, {}); b = list(calls)
-        assert a == b and sum(c[0] == "hgemm" for c in a) == 3
+    mir = _qlin(refstubs.tensors(k, n))
+    for rows, ref_calls in zip(refstubs.SLICING_ROWS, gold["slicing"]):
+        recorder.clear()
+        mir.forward(torch.zeros((rows, k), dtype=torch.half), {})
+        assert recorder == ref_calls and sum(c[0] == "hgemm" for c in ref_calls) == 3, rows
 
 
-def test_reference_multilinear_tables_match_the_mirror():
+def test_reference_multilinear_tables_match_the_mirror(gold):
     """modules/multilinear.py builds the pointer tables exl3_mgemm reads; pointer_tables must build the same ones."""
-    src = open(os.path.join(REF, "modules", "multilinear.py")).read()
-    ns = {}
-    exec(compile(src.replace("from . import Linear", "Linear = object"), "multilinear_ref", "exec"), ns)     # executed in memory, not copied
     from exllamav3_b200 import pointer_tables
+    g = gold["multilinear"]
     k, n = 128, 256
-    inners = [_qlin(_tensors(k, n)) for _ in range(3)]
-    for i in inners:
-        i.quant_type = "exl3"                                   # the attribute the reference's table builder asserts on
-
-    class Lin:                                                  # the reference wraps LinearEXL3 in modules.Linear (.inner)
-        def __init__(self, inner):
-            self.inner, self.quant_type, self.softcap, self.post_scale = inner, "exl3", 0.0, 1.0
-            self.in_features, self.out_features = inner.in_features, inner.out_features
-    ref_ml = ns["MultiLinear"]("cpu", [Lin(i) for i in inners])
-    ml = dict(zip(("ptrs_trellis", "ptrs_suh", "ptrs_svh"), pointer_tables("cpu", inners)))
-    for a in ("ptrs_trellis", "ptrs_suh", "ptrs_svh"):
-        assert torch.equal(getattr(ref_ml, a), ml[a]) and ml[a].dtype == torch.long
-    assert (ref_ml.K, ref_ml.mcg, ref_ml.mul1, ref_ml.in_features, ref_ml.out_features) == (4, False, True, k, n)
+    inners = [_qlin(refstubs.tensors(k, n)) for _ in range(3)]
+    where = {getattr(i, a).data_ptr(): [j, a] for j, i in enumerate(inners) for a in ("trellis", "suh", "svh")}
+    tables = dict(zip(("ptrs_trellis", "ptrs_suh", "ptrs_svh"), pointer_tables("cpu", inners)))
+    for a, t in tables.items():
+        assert [where[int(p)] for p in t.tolist()] == g["tables"][a] and str(t.dtype) == g["dtype"], a
+    i0 = inners[0]
+    assert [i0.K, bool(i0.mcg), bool(i0.mul1), i0.in_features, i0.out_features] == g["fields"]
 
 
-def test_every_reference_call_site_of_the_qgemm_surface_fits_the_shim():
-    """Static audit: every `ext.<op>(...)` call in the reference's Python sources, for the ops of the qgemm path, is bound
-    (by argument count and keyword names) against the shim's signature.  SURVEY.md 8b lists these callers."""
-    import ast
+def test_every_reference_call_site_of_the_qgemm_surface_fits_the_shim(gold):
+    """Every `ext.<op>(...)` call site of the qgemm surface in the reference's Python tree (recorded by an AST audit) binds,
+    by positional count and keyword names, against the shim's signature.  SURVEY.md 8b lists these callers."""
     from exllamav3_b200 import ext
-    ops = ["exl3_gemm", "exl3_mgemm", "reconstruct", "reconstruct_slice", "reconstruct_had_slice", "had_r_128", "hgemm",
-           "exl3_gemv", "g_get_cc", "g_get_num_sms", "exl3_gemv_int8_max_k", "exl3_gemm_num_kernel_shapes", "exl3_gemm_shape_compat"]
-    sigs = {o: inspect.signature(getattr(ext, o)) for o in ops}
-    seen = {o: 0 for o in ops}
-    files = 0
-    for root, _, names in os.walk(os.path.dirname(REF)):            # the package, science/ (qgemm_benchmark.py), tests/, eval/
-        if "exllamav3_ext" in root:
-            continue
-        for nm in names:
-            if not nm.endswith(".py"):
-                continue
-            path = os.path.join(root, nm)
-            try:
-                tree = ast.parse(open(path).read())
-            except SyntaxError:
-                continue
-            files += 1
-            for node in ast.walk(tree):
-                if (isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute) and node.func.attr in sigs
-                        and isinstance(node.func.value, ast.Name) and node.func.value.id == "ext"):
-                    if any(isinstance(a, ast.Starred) for a in node.args) or any(k.arg is None for k in node.keywords):
-                        continue
-                    op = node.func.attr
-                    try:
-                        sigs[op].bind(*([None] * len(node.args)), **{k.arg: None for k in node.keywords})
-                    except TypeError as e:
-                        raise AssertionError(f"{path}:{node.lineno}: ext.{op} call does not fit the shim: {e}")
-                    seen[op] += 1
-    assert files > 50
-    assert seen["exl3_gemm"] >= 1 and seen["exl3_gemm_num_kernel_shapes"] >= 1 and seen["exl3_gemm_shape_compat"] >= 1   # science/qgemm_benchmark.py
-    # the call sites SURVEY.md 8b names exist and were checked
+    seen = {o: 0 for o in refstubs.AUDIT_OPS}
+    for path, line, op, nargs, kws in gold["audit"]:
+        try:
+            inspect.signature(getattr(ext, op)).bind(*([None] * nargs), **{kw: None for kw in kws})
+        except TypeError as e:
+            raise AssertionError(f"{path}:{line}: ext.{op} call does not fit the shim: {e}")
+        seen[op] += 1
+    assert seen["exl3_gemm"] >= 1 and seen["exl3_gemm_num_kernel_shapes"] >= 1 and seen["exl3_gemm_shape_compat"] >= 1
     assert seen["exl3_mgemm"] >= 8 and seen["hgemm"] >= 3 and seen["had_r_128"] >= 2 and seen["reconstruct"] >= 2
     assert seen["reconstruct_had_slice"] >= 2 and seen["reconstruct_slice"] >= 1 and seen["exl3_gemv_int8_max_k"] >= 1
 
 
-def test_reference_use_mgemm_policy_with_the_shims_answer(monkeypatch):
-    """model/config.py:48-64, the reference's OWN policy function, evaluated with this shim's exl3_gemv_int8_max_k (0): k+v and
-    gate+up stay fused for every bitrate -- the launch list bench.py times (161 launches) -- whereas with the reference
-    extension's answer on Blackwell (6) the wide 4-bpw gate+up pair is unfused (225-launch variant, bench.py --no-fuse)."""
+def test_reference_use_mgemm_policy_with_the_shims_answer(gold, monkeypatch):
+    """model/config.py:48-64, the reference's OWN policy, recorded for the shim's exl3_gemv_int8_max_k answer (0) and for the
+    reference extension's answer on Hopper (6): with the shim, k+v and gate+up stay fused for every bitrate -- the launch list
+    bench.py times -- whereas with 6 the wide 4-bpw gate+up pair is unfused (bench.py --no-fuse)."""
     from exllamav3_b200 import ext
-
-    def mod(name, **attrs):
-        m = types.ModuleType(name); m.__path__ = []
-        for k, v in attrs.items():
-            setattr(m, k, v)
-        monkeypatch.setitem(sys.modules, name, m)
-
-    mod("exllamav3"); mod("exllamav3.model"); mod("exllamav3.util")
-    mod("exllamav3.util.rope", RopeSettings=object, RopeStyle=object)
-    mod("exllamav3.loader", SafetensorsCollection=object)
-    mod("exllamav3.util.file", read_dict=None, no_value=None, no_default=None)
-    mod("exllamav3.ext", exllamav3_ext=ext)
-    for v in ("EXL3_INT8_GEMV", "EXL3_MGEMM_K_THRESHOLD", "EXL3_MGEMM_N_THRESHOLD"):
-        monkeypatch.delenv(v, raising=False)
-    spec = importlib.util.spec_from_file_location("exllamav3.model.config", os.path.join(REF, "model", "config.py"))
-    cfg = importlib.util.module_from_spec(spec)
-    monkeypatch.setitem(sys.modules, "exllamav3.model.config", cfg)
-    spec.loader.exec_module(cfg)
-    ip = cfg.InferParams()
-    monkeypatch.setattr(ext, "_check", lambda rc: 148)                      # no device here: the index check is not under test
+    monkeypatch.setattr(ext, "_check", lambda rc: 132)                      # no device here: the index check is not under test
     assert ext.exl3_gemv_int8_max_k(0) == 0
+    policy = {(mk, K, n, mul1): fused for mk, K, n, mul1, fused in gold["use_mgemm"]}
     for K in range(1, 9):
-        assert ip.use_mgemm(K, 14336, mul1=True, device="cuda:0")          # gate/up: fused at every bitrate
-        assert ip.use_mgemm(K, 1024, mul1=True, device="cuda:0")           # k/v
-        assert ip.use_mgemm(K, 14336, mul1=False, device="cuda:0")         # other codebooks are always fused
-    monkeypatch.setattr(ext, "exl3_gemv_int8_max_k", lambda dev: 6)        # what the reference's own extension reports on sm_100
-    assert not ip.use_mgemm(4, 14336, mul1=True, device="cuda:0")          # wide 4 bpw pair: unfused there
-    assert ip.use_mgemm(4, 1024, mul1=True, device="cuda:0")               # narrow outputs stay fused either way
-    assert ip.use_mgemm(7, 14336, mul1=True, device="cuda:0")
+        for n in (1024, 14336):
+            for mul1 in (True, False):
+                assert policy[(ext.exl3_gemv_int8_max_k(0), K, n, mul1)], (K, n, mul1)     # fused at every bitrate
+    assert not policy[(6, 4, 14336, True)]                                  # wide 4 bpw pair: unfused with the reference's answer
+    assert policy[(6, 4, 1024, True)] and policy[(6, 7, 14336, True)] and policy[(6, 4, 14336, False)]
 
 
-def test_reference_tp_import_split_equals_tp_slice(ref_exl3):
-    """The reference's OWN shard construction (LinearEXL3.tp_export / tp_import_split, modules/quant/exl3.py:268-330), run with a
-    trivial in-process stand-in for its SHM producer / consumer transport, against this repo's tp.tp_slice."""
-    ref_mod, _ = ref_exl3
+def test_reference_tp_import_split_equals_tp_slice(gold):
+    """The reference's OWN shard construction (LinearEXL3.tp_export / tp_import_split, modules/quant/exl3.py:268-330) for every
+    split of world 3, against this repo's tp.tp_slice on the same inputs."""
     from exllamav3_b200 import tp
-
-    class Producer:
-        def send(self, t): return t
-
-    class Consumer:
-        def recv(self, t, cuda=False, slice_dim=None, first=None, last=None):
-            if t is None:
-                return None
-            return t if slice_dim is None else t.narrow(slice_dim, first, last - first).contiguous()
-
+    g = gold["tp"]
     k, n = 512, 768
-    tens = _tensors(k, n)
-    g = torch.Generator().manual_seed(5)
-    tens["suh"] = torch.randn(k, generator=g).half(); tens["svh"] = torch.randn(n, generator=g).half()
-    bias = torch.randn(n, generator=g).half()
-    ref_full = ref_mod.LinearEXL3(None, k, n, bias=bias, out_dtype=torch.float, **tens)
-    mir_full = _qlin(tens, bias=bias, out_dtype=torch.float)
-    exported = ref_full.tp_export(None, Producer())
-    ctx = {"consumer": Consumer(), "device": "cpu"}
+    tens, bias = refstubs.tp_tensors(k, n)
+    assert {a: refstubs.digest(tens[a]) for a in ("trellis", "suh", "svh")} | {"bias": refstubs.digest(bias)} == g["inputs"]
+    mir = _qlin(tens, bias=bias, out_dtype=torch.float)
     world = 3
-    splits = [(True, a, b) for (a, b) in tp.split_ranges(n, world)] + [(False, a, b) for (a, b) in tp.split_ranges(k, world)] + [None]
-    for split in splits:
-        r = ref_mod.LinearEXL3.tp_import_split(ctx, exported, None, split)
-        m = tp.tp_slice(mir_full, split)
-        assert (r.in_features, r.out_features, r.K, r.mcg, r.mul1, r.out_dtype) == (m.in_features, m.out_features, m.K, m.mcg, m.mul1, m.out_dtype)
-        assert torch.equal(r.trellis, m.trellis) and torch.equal(r.suh, m.suh) and torch.equal(r.svh, m.svh)
-        assert (r.bias is None) == (m.bias is None) and (r.bias is None or torch.equal(r.bias, m.bias))
+    splits = [[True, a, b] for (a, b) in tp.split_ranges(n, world)] + [[False, a, b] for (a, b) in tp.split_ranges(k, world)] + [None]
+    assert splits == [s["split"] for s in g["shards"]]
+    for split, ref in zip(splits, g["shards"]):
+        m = tp.tp_slice(mir, tuple(split) if split else None)
+        assert [m.in_features, m.out_features, m.K, bool(m.mcg), bool(m.mul1), str(m.out_dtype)] == ref["fields"], split
+        for a in ("trellis", "suh", "svh", "bias"):
+            assert refstubs.digest(getattr(m, a)) == ref[a], (split, a)
         assert m.trellis.is_contiguous()

@@ -3,9 +3,8 @@ Row-parallel GEMM with the tensor-parallel sum fused into its epilogue (csrc/gem
 
 CPU part (always runs): eligibility rules, argument validation, the host-side selection in tp.row_parallel_forward.
 
-GPU part (verified on a B200 in round 2, gpurun_out/r02_call1): world-1 equality with the plain kernel and the loop-back
-protocol test run on one GPU (-m gpu); the two-process test needs two GPUs and carries the `multigpu` marker instead
-(gpurun --gpus 2 -- python -m pytest tests -m multigpu).
+GPU part: world-1 equality with the plain kernel and the loop-back protocol test run on one GPU (-m gpu); the two-process
+test needs two GPUs and carries the `multigpu` marker instead (python -m pytest tests -m multigpu on a two-GPU machine).
 """
 import ctypes, os
 import numpy as np

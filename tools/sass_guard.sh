@@ -3,7 +3,7 @@
 #   bash tools/sass_guard.sh save  [dir]     after a build of the known-good tree     (default dir: /tmp/exl3b_sass)
 #   bash tools/sass_guard.sh check [dir]     after rebuilding the modified tree: prints differing SASS lines per object
 # Lines that differ only in constant-bank-4 offsets (addresses of printf format strings) and the file-name / function header lines
-# are ignored.  New objects (no snapshot) are reported as such.  Used throughout the end of round 1 (DESIGN.md, status paragraph).
+# are ignored.  New objects (no snapshot) are reported as such.
 set -u
 mode=${1:-check}; dir=${2:-/tmp/exl3b_sass}
 objs=exllamav3_b200/build
