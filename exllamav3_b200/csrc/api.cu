@@ -244,15 +244,15 @@ int exl3b_gemm_plan(int m, int k, int n, int K, int cb, int num_sms, int force_n
 
 int exl3b_plan_unit_range(int64_t units, int grid, int cta, int64_t* begin, int64_t* end)
 {
-    EXL3B_CHECK(units >= 1 && grid >= 1 && grid <= units && cta >= 0 && cta < grid && begin && end, EXL3B_ERR_ARG, "exl3_plan_unit_range: bad argument");
-    *begin = unit_begin(units, grid, cta); *end = unit_begin(units, grid, cta + 1);
+    EXL3B_CHECK(units >= 1 && grid >= 1 && grid <= units && partition_fits(units, grid) && cta >= 0 && cta < grid && begin && end, EXL3B_ERR_ARG, "exl3_plan_unit_range: bad argument");
+    *begin = unit_begin((int) units, grid, cta); *end = unit_begin((int) units, grid, cta + 1);
     return 0;
 }
 
 int exl3b_plan_cta_of_unit(int64_t units, int grid, int64_t unit)
 {
-    EXL3B_CHECK(units >= 1 && grid >= 1 && grid <= units && unit >= 0 && unit < units, EXL3B_ERR_ARG, "exl3_plan_cta_of_unit: bad argument");
-    return cta_of_unit(units, grid, unit);
+    EXL3B_CHECK(units >= 1 && grid >= 1 && grid <= units && partition_fits(units, grid) && unit >= 0 && unit < units, EXL3B_ERR_ARG, "exl3_plan_cta_of_unit: bad argument");
+    return cta_of_unit((int) units, grid, (int) unit);
 }
 
 int exl3b_gemm(void* stream_, const void* A, const void* B, void* C, const void* suh, void* A_had, const void* svh,

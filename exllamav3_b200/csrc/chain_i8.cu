@@ -123,13 +123,13 @@ struct Cursor
             const long long U = stages[stage].U;
             Gs = U < G ? (int) U : G;
             if (cta >= Gs) continue;
-            const long long ub = unit_begin(U, Gs, cta), ue = unit_begin(U, Gs, cta + 1);
+            const long long ub = unit_begin((int) U, Gs, cta), ue = unit_begin((int) U, Gs, cta + 1);
             u = ub; uend = ue;
             op = stages[stage].op_begin;
             while (u >= ops[op].unit_off + (long long) ops[op].KB * ops[op].strips) ++op;
             KB = ops[op].KB; strips = ops[op].strips;
-            const long long rel = u - ops[op].unit_off;
-            strip = (int) (rel / KB); kb = (int) (rel - (long long) strip * KB);
+            const int rel = (int) (u - ops[op].unit_off);
+            strip = rel / KB; kb = rel - strip * KB;
             start_run();
             valid = true;
             return;
@@ -235,7 +235,15 @@ __device__ __forceinline__ void ch_watchdog(uint32_t& polls, unsigned long long&
         unsigned long long t;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
         if (t0 == 0) t0 = t;
-        else if (t - t0 > 4000000000ull) { printf("exl3b chain: %s timeout (block %d, %d, %d)\n", what, blockIdx.x, a, b); __trap(); }
+        else if (t - t0 > 4000000000ull)
+        {
+#ifdef EXL3B_TC_DEBUG
+            printf("exl3b chain: %s timeout (block %d, %d, %d)\n", what, blockIdx.x, a, b);
+#else
+            (void) what; (void) a; (void) b;
+#endif
+            __trap();
+        }
     }
 }
 
@@ -464,11 +472,12 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                 for (int r = 0; r < CH_MR; ++r)
                 {
                     // bound on |xh|: block 2-norm, + margin for the fp32 reduction and the fp16 rounding of xh
-                    const float bnd = sqrtf(__uint_as_float(s_norm2[r])) * 1.002f;
-                    inv_scale[r] = bnd > 0.f ? (float) I8_QMAX / bnd : 0.f;
+                    const float n2 = __uint_as_float(s_norm2[r]);
+                    const float bnd = (n2 > 0.f ? i8_sqrt_rn(n2) : 0.f) * 1.002f;   // n2: 0 or in [2^-48, 2^40]
+                    inv_scale[r] = bnd > 0.f ? i8_qmax_over(bnd) : 0.f;
                     // every digit warp stores the (identical) value before its own first X_FULL arrive of this op: whichever
                     // arrive the MMA side observes, the scale the epilogue reads later is ordered before it
-                    if (lane == r) s_scale[(cur_op % CH_SCALE_SLOTS) * CH_MR + r] = bnd / (float) I8_QMAX;
+                    if (lane == r) s_scale[(cur_op % CH_SCALE_SLOTS) * CH_MR + r] = i8_over_qmax(bnd);
                 }
                 CH_STAMP(warp == CH_XF_WARP0 && lane == 0 && c.seq == 0, 60);
             }
@@ -659,7 +668,7 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
 
             // who else holds k-segments of this strip?
             const long long gs = o.unit_off + (long long) strip * o.KB;
-            const int c_a = cta_of_unit(U, c.Gs, gs), c_b = cta_of_unit(U, c.Gs, gs + o.KB - 1);
+            const int c_a = cta_of_unit((int) U, c.Gs, (int) gs), c_b = cta_of_unit((int) U, c.Gs, (int) (gs + o.KB - 1));
             const bool full = c_a == c_b;
             bool emit = full;
             if (full)
@@ -833,6 +842,7 @@ static int chain_build(const exl3b_chain_op* in, int n_ops, int num_sms, Chain& 
     int grid = num_sms;
     if (Umax < grid) grid = (int) Umax;
     EXL3B_CHECK(grid <= DevCtx::I8_PART_CTAS, EXL3B_ERR_UNSUPPORTED, "exl3_chain: grid exceeds the split-K exchange buffer");
+    EXL3B_CHECK(partition_fits(Umax, grid), EXL3B_ERR_UNSUPPORTED, "exl3_chain: too many units for the 32-bit stream-K partition");
     ch.p = ChainParams{};
     ch.p.n_ops = n_ops; ch.p.n_stages = (int) ch.stages.size();
     ch.p.S = S; ch.p.w_bytes = w_bytes; ch.p.cache_bytes = (int) cache; ch.p.suh_bytes = (int) suhb;

@@ -147,10 +147,10 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
     // ---- this CTA's unit range ----
     const int KB = p.k / 128;
     const int strips = p.n / 128;
-    const long long U = (long long) KB * strips;
+    const int U = KB * strips;
     const int G = gridDim.x;
-    const long long ubeg = unit_begin(U, G, blockIdx.x), uend = unit_begin(U, G, blockIdx.x + 1);
-    const int n_units = (int) (uend - ubeg);
+    const int ubeg = unit_begin(U, G, blockIdx.x), uend = unit_begin(U, G, blockIdx.x + 1);
+    const int n_units = uend - ubeg;
 
     if (warp == 0)
     {
@@ -178,7 +178,7 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
             }
         };
         const int pre = n_units < S ? n_units : S;
-        const int strip0 = (int) (ubeg / KB), kb0 = (int) (ubeg % KB);
+        const int strip0 = ubeg / KB, kb0 = ubeg % KB;
         int strip = strip0, kb = kb0;
         auto next_unit = [&] { if (++kb == KB) { kb = 0; ++strip; } };
         for (int u = 0; u < pre; ++u) { issue_w(u, strip, kb); next_unit(); }   // weights never depend on the previous kernel
@@ -207,7 +207,7 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
         {
             pdl_wait();                                  // A is produced by the previous kernel
             const int xw = warp - TC_XF_WARP0;           // 0 / 1: units of alternating parity
-            int kb = (int) ((ubeg + xw) % KB);
+            int kb = (ubeg + xw) % KB;
             int s = xw % S, ph = 0;
             if (xw >= S) { s = 0; ph = 1; }              // S >= 2 always
             const int kstep = 2 % KB;
@@ -274,11 +274,11 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
         int u = 0;
         while (u < n_units)
         {
-            const long long g = ubeg + u;
-            const int strip = (int) (g / KB), kb = (int) (g % KB);
+            const int g = ubeg + u;
+            const int strip = g / KB, kb = g % KB;
             const int to_strip_end = KB - kb;
             const int seg = (n_units - u) < to_strip_end ? (n_units - u) : to_strip_end;
-            const long long gs = (long long) strip * KB;
+            const int gs = strip * KB;
             const int c_a = cta_of_unit(U, G, gs), c_b = cta_of_unit(U, G, gs + KB - 1);
             const int n_contrib = c_b - c_a + 1;
             const bool full = n_contrib == 1;
@@ -542,6 +542,7 @@ int plan_gemm_tc(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* 
     EXL3B_CHECK((size_t) 2 * grid * NT * 128 * 4 <= DevCtx::WS_BYTES_PER_SLOT, EXL3B_ERR_UNSUPPORTED,
                 "exl3_gemm: split-K workspace too small");
     EXL3B_CHECK(n / 128 <= DevCtx::COUNTERS_PER_SLOT, EXL3B_ERR_UNSUPPORTED, "exl3_gemm: too many column strips");
+    EXL3B_CHECK(partition_fits(U, grid), EXL3B_ERR_UNSUPPORTED, "exl3_gemm: too many units for the 32-bit stream-K partition");
     pl->rows = NT; pl->stages = stages; pl->b_bytes = b_bytes; pl->smem_total = L.total; pl->grid = grid; pl->units = U;
     return 0;
 }

@@ -66,6 +66,7 @@ int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPla
     if (grid > U) grid = (int) U;
     EXL3B_CHECK(n / 128 <= DevCtx::COUNTERS_PER_SLOT, EXL3B_ERR_UNSUPPORTED, "exl3_gemm: too many column strips");
     EXL3B_CHECK(grid <= DevCtx::I8_PART_CTAS, EXL3B_ERR_UNSUPPORTED, "exl3_gemm (i8): grid exceeds the split-K exchange buffer");
+    EXL3B_CHECK(partition_fits(U, grid), EXL3B_ERR_UNSUPPORTED, "exl3_gemm (i8): too many units for the 32-bit stream-K partition");
     pl->rows = MR; pl->stages = stages; pl->b_bytes = i8_b_stage(MR); pl->b_load_bytes = cache_bytes; pl->smem_total = L.total;
     pl->grid = grid; pl->units = U; pl->a_stages = 0; pl->d_bufs = 2; pl->tmem_cols = 0;
     return 0;
@@ -113,6 +114,7 @@ int plan_fanout_groups(int k, const int32_t* widths, int mats, int num_sms, int*
     {
         if (widths[j] < 128 || widths[j] % 128) return 0;
         U[j] = (long long) (k / 128) * (widths[j] / 128); Utot += U[j];
+        if (!partition_fits(U[j], num_sms)) return 0;
     }
     int grid = num_sms; if (grid > Utot) grid = (int) Utot;
     long long Urem = Utot; int Grem = grid; cta0[0] = 0;
@@ -182,6 +184,7 @@ int launch_mgemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a)
     const long long U = (long long) (a.k / 128) * (a.n / 128);
     int gpm = ctx->num_sms / mats;
     if (gpm > U) gpm = (int) U;
+    EXL3B_CHECK(partition_fits(U, gpm), EXL3B_ERR_UNSUPPORTED, "exl3_mgemm (i8): too many units for the 32-bit stream-K partition");
     p.g_per_mat = gpm;
     int grid = gpm * mats;
     if (a.size_n_list)

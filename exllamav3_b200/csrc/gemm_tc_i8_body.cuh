@@ -125,6 +125,20 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         if (p.rag) Cout = reinterpret_cast<char*>(p.c_ptrs[mat]); else Cout += (size_t) slot * p.c_mat_stride;
     }
 
+    if (multi && warp == 0)
+    {
+        // per-CTA tensor map: the template (dims / strides / box of this shape) with matrix `mat`'s address -- and, in a fan-out
+        // launch, its own width (innermost extent in 8-byte elements, row pitch in bytes).  Patched here, where `mat` is at
+        // hand, so that it is not kept live until the producer's loop (it was spilled there).
+        const size_t w_pitch = (size_t) (n_loc / 16) * 32 * K;           // bytes per 16-row tile row of the packed tensor
+        uint8_t* stm = smem + ((L.off_bars + 640 + 127) & ~127);
+        reinterpret_cast<uint32_t*>(stm)[lane] = reinterpret_cast<const uint32_t*>(tmap_w)[lane];
+        __syncwarp();
+        void* gtm = p.tmap_slots + (size_t) blockIdx.x * 128;
+        if (p.rag) tmap_patch_address_width(smem_u32(stm), gtm, p.B_ptrs[mat], (uint32_t) (w_pitch / 8), (uint64_t) w_pitch, lane);
+        else tmap_patch_address(smem_u32(stm), gtm, p.B_ptrs[mat], lane);
+    }
+
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
     const uint32_t bar0 = smem_u32(bars);
     auto W_FULL = [&](int s) { return bar0 + 8u * s; };
@@ -173,9 +187,9 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
 
     const int KB = p.k / 128;
     const int strips = n_loc / 128;
-    const long long U = (long long) KB * strips;
-    const long long ubeg = unit_begin(U, G, cta), uend = unit_begin(U, G, cta + 1);
-    const int n_units = (int) (uend - ubeg);
+    const int U = KB * strips;
+    const int ubeg = unit_begin(U, G, cta), uend = unit_begin(U, G, cta + 1);
+    const int n_units = uend - ubeg;
 
     // fp16 transformed activation of (row r, k-block kb), 4 values per lane, exactly as the reference's A_had
     auto xh_finish = [&](uint2 raw, uint2 scb, float (&v)[4])
@@ -291,24 +305,12 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     if (warp == 0)
     {
         // =========================== producer ===========================
-        const void* tm = tmap_w;
-        const size_t w_pitch = (size_t) (n_loc / 16) * 32 * K;               // bytes per 16-row tile row of the packed tensor
-        if (multi)
-        {
-            // per-CTA tensor map: the template (dims / strides / box of this shape) with matrix `mat`'s address -- and, in a fan-out
-            // launch, its own width (innermost extent in 8-byte elements, row pitch in bytes)
-            uint8_t* stm = smem + ((L.off_bars + 640 + 127) & ~127);
-            reinterpret_cast<uint32_t*>(stm)[lane] = reinterpret_cast<const uint32_t*>(tmap_w)[lane];
-            __syncwarp();
-            void* gtm = p.tmap_slots + (size_t) blockIdx.x * 128;
-            if (p.rag) tmap_patch_address_width(smem_u32(stm), gtm, p.B_ptrs[mat], (uint32_t) (w_pitch / 8), (uint64_t) w_pitch, lane);
-            else tmap_patch_address(smem_u32(stm), gtm, p.B_ptrs[mat], lane);
-            tm = gtm;
-        }
-        else if (elect_one()) prefetch_tmap(tmap_w);
+        // multi-matrix launch: this CTA's tensor map was patched at the top of the kernel
+        const void* tm = multi ? static_cast<const void*>(p.tmap_slots + (size_t) blockIdx.x * 128) : static_cast<const void*>(tmap_w);
+        if (!multi && elect_one()) prefetch_tmap(tmap_w);
         const uint64_t pol_w = policy_evict_first();
         const uint32_t w_smem0 = smem_u32(smem);
-        int strip = (int) (ubeg / KB), kb = (int) (ubeg % KB);
+        int strip = ubeg / KB, kb = ubeg % KB;
         int s = 0, ph = 0;
         for (int u = 0; u < n_units; ++u)
         {
@@ -335,9 +337,9 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         for (int r = 0; r < MR; ++r)
         {
             const float mx = __uint_as_float(s_absmax[r]);
-            inv_scale[r] = mx > 0.f ? (float) I8_QMAX / mx : 0.f;
+            inv_scale[r] = mx > 0.f ? i8_qmax_over(mx) : 0.f;
         }
-        int kb = (int) ((ubeg + xw) % KB);
+        int kb = (ubeg + xw) % KB;
         int s = xw % S, ph = 0;
         const int kstep = 2 % KB;
         for (int u = xw; u < n_units; u += 2)
@@ -418,7 +420,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         for (int i = 0; i < MR; ++i) acc[i] = 0u;
         int t_lo = 0, t_hi = 0;                          // digit sums of activation rows c and c + 4 over the group's units
         int s = 0, sph = 0, dbuf = 0, dphase = 0, seg_left = 0, sub_left = 0;
-        int kb = (int) (ubeg % KB);
+        int kb = ubeg % KB;
         for (int u = 0; u < n_units; ++u)
         {
             if (seg_left == 0)
@@ -432,9 +434,6 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                 mbar_wait<32>(W_FULL(s), sph);
                 if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) stamp(3);
                 const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
-                uint32_t w[2][K + 1];
-                #pragma unroll
-                for (int r = 0; r < 2; ++r) load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, w[r]);
                 mbar_wait(X_FULL(s), sph);                                   // the unit's activation digits
                 const int* dsum = reinterpret_cast<const int*>(smem + L.off_b + s * L.b_bytes + I8_B_BYTES);
                 if (c < p.m) t_lo += dsum[c];
@@ -443,9 +442,11 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                 #pragma unroll
                 for (int r = 0; r < 2; ++r)
                 {
-                    uint32_t o0[16], o1[16];
-                    decode16_i8<K, 0>(w[r], o0);
-                    decode16_i8<K, 1>(w[r], o1);
+                    // the weight words of k-half r are loaded only now: one k-half's words and fragments are live at a time
+                    uint32_t w[K + 1], o0[16], o1[16];
+                    load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, w);
+                    decode16_i8<K, 0>(w, o0);
+                    decode16_i8<K, 1>(w, o1);
                     #pragma unroll
                     for (int i = 0; i < MR; ++i) reg_fence(acc[i]);
                     wgmma_fence();
@@ -597,7 +598,9 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                             if (t0 == 0) t0 = t;
                             else if (t - t0 > 20000000000ull)
                             {
+#ifdef EXL3B_TC_DEBUG
                                 if (lane == 0) printf("exl3b: tensor-parallel exchange timeout (rank %d block %d strip %d have %x)\n", rank, blockIdx.x, strip, have);
+#endif
                                 __trap();
                             }
                         }
@@ -632,11 +635,11 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         int u = 0;
         while (u < n_units)
         {
-            const long long g = ubeg + u;
-            const int strip = (int) (g / KB), kb = (int) (g % KB);
+            const int g = ubeg + u;
+            const int strip = g / KB, kb = g % KB;
             const int to_strip_end = KB - kb;
             const int seg = (n_units - u) < to_strip_end ? (n_units - u) : to_strip_end;
-            const long long gs = (long long) strip * KB;
+            const int gs = strip * KB;
             const int c_a = cta_of_unit(U, G, gs), c_b = cta_of_unit(U, G, gs + KB - 1);
             const int n_contrib = c_b - c_a + 1;
             const bool full = n_contrib == 1;
@@ -660,7 +663,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                         // sum_k q_k (bytesum_kn - 510), exact in 64-bit (the two groups' int32 partials add without loss)
                         const long long sp = i8_centred_sum(d0[2 * r] + d1[2 * r], d0[2 * r + 1] + d1[2 * r + 1], T);
                         const float mx = __uint_as_float(s_absmax[r]);
-                        const float scale = mx / (float) I8_QMAX;
+                        const float scale = i8_over_qmax(mx);
                         facc[r] += i8_assemble(sp, T, scale, k_inv, c1);
                     }
                 }
@@ -728,7 +731,13 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                                     unsigned long long t;
                                     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
                                     if (t0 == 0) t0 = t;
-                                    else if (t - t0 > 4000000000ull) { printf("exl3b: split-K exchange timeout (block %d strip %d)\n", blockIdx.x, strip); __trap(); }
+                                    else if (t - t0 > 4000000000ull)
+                                    {
+#ifdef EXL3B_TC_DEBUG
+                                        printf("exl3b: split-K exchange timeout (block %d strip %d)\n", blockIdx.x, strip);
+#endif
+                                        __trap();
+                                    }
                                 }
                             } while (!ok);
                             #pragma unroll

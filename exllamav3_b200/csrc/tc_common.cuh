@@ -91,8 +91,18 @@ __host__ __device__ inline TcSmemLayout tc_smem_layout(int K, int b_bytes, int s
 
 // ---- work partition helpers -------------------------------------------------------------------------------------
 // (host + device: the CPU tests walk the same partition the kernels use, exl3b_plan_* in api.cu)
-__host__ __device__ __forceinline__ long long unit_begin(long long U, int G, int c) { return U * c / G; }
-__host__ __device__ __forceinline__ int cta_of_unit(long long U, int G, long long g) { return (int) (((g + 1) * G - 1) / U); }
+// 32-bit arithmetic: a 64-bit division is a subroutine call in SASS, and a call inside a kernel that issues wgmma makes
+// ptxas serialize every wgmma of it.  The planners only launch grids for which partition_fits(U, G) holds, so U * c and
+// (g + 1) * G - 1 (c <= G, g < U) never exceed 32 unsigned bits.
+__host__ __device__ __forceinline__ bool partition_fits(long long U, long long G)
+{
+    return U >= 1 && G >= 1 && U <= 0x7fffffffll && U * G <= 0xffffffffll;
+}
+__host__ __device__ __forceinline__ int unit_begin(int U, int G, int c) { return (int) ((uint32_t) U * (uint32_t) c / (uint32_t) G); }
+__host__ __device__ __forceinline__ int cta_of_unit(int U, int G, int g)
+{
+    return (int) ((((uint32_t) g + 1u) * (uint32_t) G - 1u) / (uint32_t) U);
+}
 
 
 int get_weight_tmap(const void* B, int k, int n, int K, CUtensorMap* out);
