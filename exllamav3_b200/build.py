@@ -26,8 +26,10 @@ NVCC_FLAGS = [
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
 ]
-if os.environ.get("EXL3B_TC_DEBUG", "0") != "0":       # bring-up build: in-kernel timeline stamps + experiment knobs
-    NVCC_FLAGS.append("-DEXL3B_TC_DEBUG")
+# bring-up build: in-kernel timeline stamps + experiment knobs; EXL3B_TC_DEBUG=2 also prints the timeout messages of the
+# bounded waits (a function call: ptxas then serializes the wgmma of the int8 decode-GEMM, so level 1 is the one to time)
+if os.environ.get("EXL3B_TC_DEBUG", "0") != "0":
+    NVCC_FLAGS.append("-DEXL3B_TC_DEBUG=" + os.environ["EXL3B_TC_DEBUG"])
 
 
 if os.environ.get("EXL3B_NVCC_EXTRA"):                   # extra nvcc flags, e.g. EXL3B_NVCC_EXTRA="-Xptxas -warn-spills" (+ -f)

@@ -83,7 +83,10 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     int* const s_dt = reinterpret_cast<int*>(smem + L.off_d + i8_d_bytes(MR) - 2 * 2 * 8 * 4);   // digit sums, [dbuf][group][8]
     const bool cached = p.b_load_bytes > 0;                            // host: cache_bytes (0 = recompute per unit)
     half* xh_cache = reinterpret_cast<half*>(smem + L.total);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    // warp index broadcast from lane 0: ptxas then knows it is warp-uniform, so the role branches and everything derived from
+    // the warp index (decode group, stage, wgmma descriptors) stay in uniform registers; a descriptor in per-thread registers
+    // costs a 64-bit add and two R2UR in front of every wgmma (tests/test_i8_issue_sass_host.py)
+    const int warp = __shfl_sync(0xffffffffu, (int) (threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
     const int S = p.stages;
 
     // multi-matrix launch (exl3_mgemm): group `mat` of g_per_mat CTAs works on matrix `mat` exactly like a single-matrix
@@ -598,7 +601,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                             if (t0 == 0) t0 = t;
                             else if (t - t0 > 20000000000ull)
                             {
-#ifdef EXL3B_TC_DEBUG
+#if EXL3B_TC_DEBUG >= 2
                                 if (lane == 0) printf("exl3b: tensor-parallel exchange timeout (rank %d block %d strip %d have %x)\n", rank, blockIdx.x, strip, have);
 #endif
                                 __trap();
@@ -733,7 +736,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                                     if (t0 == 0) t0 = t;
                                     else if (t - t0 > 4000000000ull)
                                     {
-#ifdef EXL3B_TC_DEBUG
+#if EXL3B_TC_DEBUG >= 2
                                         printf("exl3b: split-K exchange timeout (block %d strip %d)\n", blockIdx.x, strip);
 #endif
                                         __trap();

@@ -64,8 +64,9 @@ __device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity)
 // activity wakes the warp, so iteration counts say nothing about elapsed time.
 // BACKOFF_NS > 0: exponential back-off (BACKOFF_NS, 2x, ... capped at 16x) between polls for roles whose waits can be
 // long: polling warps otherwise burn issue slots the decode warps need.
-// The timeout message is printed only in the bring-up build (EXL3B_TC_DEBUG): printf is a function call, and any call in a
-// kernel that issues wgmma makes ptxas wait for every wgmma on its own (C7510); the trap alone still ends the launch with an error.
+// The timeout message is printed only in the bring-up build with messages (EXL3B_TC_DEBUG=2): printf is a function call, and any
+// call in a kernel that issues wgmma makes ptxas wait for every wgmma on its own (C7510), so the timeline build
+// (EXL3B_TC_DEBUG=1) leaves it out to time the production MMA schedule; the trap alone still ends the launch with an error.
 template <int BACKOFF_NS = 0>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
 {
@@ -83,7 +84,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
             if (t0 == 0) t0 = t;
             else if (t - t0 > 4000000000ull)
             {
-#ifdef EXL3B_TC_DEBUG
+#if EXL3B_TC_DEBUG >= 2
                 printf("exl3b: mbarrier timeout (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
 #endif
                 __trap();
