@@ -414,6 +414,63 @@ int exl3b_chain_run(void* stream, void* chain) { return chain_run((cudaStream_t)
 
 int exl3b_chain_destroy(void* chain) { return chain_destroy(chain); }
 
+int exl3b_moe_max_concurrency(int device)
+{
+    const int sms = exl3b_num_sms(device);
+    return sms < 0 ? sms : sms / 8;
+}
+
+int exl3b_moe_plan(const int64_t* expert_count_host, int num_experts, int max_tokens, int num_positions, int hidden,
+                   int intermediate, struct exl3b_moe_plan* out, int32_t* passes_out, int32_t* pos_code_out)
+{
+    return moe_plan_host(expert_count_host, num_experts, max_tokens, num_positions, hidden, intermediate, out, passes_out,
+                         pos_code_out);
+}
+
+// validation of exllamav3_ext/quant/exl3_moe.cu:143-200 that needs no tensor types, plus this library's own limits
+int exl3b_moe(void* stream, const void* hidden_state, void* output_state,
+              const int64_t* expert_count, const int64_t* token_sorted, const void* weight_sorted,
+              int bsz, int hidden, int intermediate, int num_experts, int num_positions, int max_tokens, int concurrency,
+              int act_function, int K_gate, int K_up, int K_down,
+              const uint64_t* gate_trellis, const uint64_t* gate_suh, const uint64_t* gate_svh,
+              const uint64_t* up_trellis, const uint64_t* up_suh, const uint64_t* up_svh,
+              const uint64_t* down_trellis, const uint64_t* down_suh, const uint64_t* down_svh,
+              int gate_mcg, int gate_mul1, int up_mcg, int up_mul1, int down_mcg, int down_mul1,
+              float act_limit, int num_active)
+{
+    if (num_active == 0) return EXL3B_TAG_NOP;
+    EXL3B_CHECK(gate_mcg == up_mcg && up_mcg == down_mcg && gate_mul1 == up_mul1 && up_mul1 == down_mul1, EXL3B_ERR_ARG,
+                "MoE kernel: gate/up/down must share the same codebook");
+    EXL3B_CHECK((gate_mcg != 0) != (gate_mul1 != 0), EXL3B_ERR_ARG, "MoE kernel: Only mcg and mul1 codebooks are supported");
+    EXL3B_CHECK(act_function >= 0 && act_function <= 2, EXL3B_ERR_ARG, "exl3_moe: act_function must be 0 (SiLU), 1 (GELU) or 2 (ReLU^2), got %d", act_function);
+    for (int K : {K_gate, K_up, K_down}) EXL3B_CHECK(K >= 1 && K <= 8, EXL3B_ERR_ARG, "K must be 1..8, got %d", K);
+    EXL3B_CHECK(bsz >= 0 && num_positions >= 0 && max_tokens >= 1 && concurrency >= 1, EXL3B_ERR_SHAPE, "exl3_moe: bad sizes");
+    EXL3B_CHECK(hidden >= 128 && hidden % 128 == 0, EXL3B_ERR_SHAPE, "exl3_moe: hidden size (%d) must be divisible by 128", hidden);
+    EXL3B_CHECK(intermediate >= 128 && intermediate % 128 == 0, EXL3B_ERR_SHAPE,
+                "exl3_moe: intermediate size (%d) must be divisible by 128", intermediate);
+    EXL3B_CHECK(num_experts >= 1 && num_experts <= MOE_MAX_EXPERTS, EXL3B_ERR_UNSUPPORTED,
+                "exl3_moe: 1..%d experts supported, got %d", MOE_MAX_EXPERTS, num_experts);
+    EXL3B_CHECK(hidden_state && output_state && expert_count && token_sorted && weight_sorted && gate_trellis && gate_suh
+                && gate_svh && up_trellis && up_suh && up_svh && down_trellis && down_suh && down_svh, EXL3B_ERR_ARG,
+                "exl3_moe: null tensor");
+    EXL3B_CHECK(((uintptr_t) hidden_state & 7) == 0 && ((uintptr_t) output_state & 15) == 0, EXL3B_ERR_ARG,
+                "exl3_moe: hidden_state must be 8-byte and output_state 16-byte aligned");
+    DevCtx* ctx; int r = get_ctx(&ctx); if (r) return r;
+    EXL3B_CHECK((long long) concurrency * 8 <= ctx->num_sms, EXL3B_ERR_ARG, "Concurrency too high for device num_sms");
+    if (bsz == 0 || num_positions == 0) return EXL3B_TAG_NOP;
+    MoeArgs a{};
+    a.hidden_state = (const half*) hidden_state; a.output_state = (float*) output_state;
+    a.expert_count = expert_count; a.token_sorted = token_sorted; a.weight_sorted = (const half*) weight_sorted;
+    a.bsz = bsz; a.hidden = hidden; a.inter = intermediate; a.num_experts = num_experts; a.num_positions = num_positions;
+    a.max_tokens = max_tokens; a.act = act_function; a.act_limit = act_limit;
+    a.K_gate = K_gate; a.K_up = K_up; a.K_down = K_down; a.cb = gate_mul1 ? 2 : 1;
+    a.gate_trellis = gate_trellis; a.gate_suh = gate_suh; a.gate_svh = gate_svh;
+    a.up_trellis = up_trellis; a.up_suh = up_suh; a.up_svh = up_svh;
+    a.down_trellis = down_trellis; a.down_suh = down_suh; a.down_svh = down_svh;
+    a.num_active = num_active;
+    return launch_moe((cudaStream_t) stream, ctx, a);
+}
+
 int exl3b_hgemm(void* stream, const void* a, const void* b, void* c, int m, int k, int n, int c_fp32,
                 int64_t c_stride)
 {

@@ -171,6 +171,25 @@ int launch_mgemm_tc_i8_routed(cudaStream_t stream, DevCtx* ctx, const MGemmArgs&
 int launch_hgemm(cudaStream_t stream, const half* a, const half* b, void* c, int m, int k, int n, bool c_fp32,
                  int64_t c_stride);
 
+// fused routed-expert MLP (moe_tc.cu, tag EXL3B_TAG_TC_MOE)
+constexpr int MOE_MAX_ROWS = 128;            // rows of one pass (the decode-GEMM's activation operand)
+constexpr int MOE_MAX_EXPERTS = 2048;
+// one pass: up to MOE_MAX_ROWS consecutive positions of one expert; row0 = its first row in chunk `chunk` of the work area
+struct MoePass { int expert, pos0, rows, row0, chunk; };
+struct MoeArgs
+{
+    const half* hidden_state; float* output_state;
+    const int64_t* expert_count; const int64_t* token_sorted; const half* weight_sorted;
+    int bsz, hidden, inter, num_experts, num_positions, max_tokens;
+    int act; float act_limit;
+    int K_gate, K_up, K_down, cb;
+    const uint64_t *gate_trellis, *gate_suh, *gate_svh, *up_trellis, *up_suh, *up_svh, *down_trellis, *down_suh, *down_svh;
+    int num_active;
+};
+int launch_moe(cudaStream_t stream, DevCtx* ctx, const MoeArgs& a);
+int moe_plan_host(const int64_t* count, int E, int T, int N, int hidden, int inter, struct exl3b_moe_plan* out, int32_t* passes_out,
+                  int32_t* pos_code_out);
+
 // ---- (K, cb) template dispatch ---------------------------------------------------------------------------------
 #define EXL3B_DISPATCH_K_CB(FN, K, cb, ...)                                                        \
     do { switch ((cb) * 8 + (K) - 1) {                                                             \

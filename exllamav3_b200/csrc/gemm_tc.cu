@@ -35,25 +35,7 @@ namespace exl3b {
 
 using namespace ptx;
 
-// ---- input transform into the tiled activation layout ---------------------------------------------------------
-// Tile of one unit: [NT / 8 row groups][16 K-chunks][8 rows][8 fp16], K-chunks 128 B apart, row groups 2048 B apart.  K order:
-// k = 16 kt + 4 j + 2 h + e (kt = 4 r + c) sits in K-chunk 2 (4 r + j) + h at element 2 c + e, i.e. lane l's four values
-// k = 4 l .. 4 l + 3 go to K-chunks 8 (l / 16) + 2 (l % 4) (+1 for the second pair), element pair (l / 4) % 4.
-__device__ __forceinline__ int xt_tile_offset(int r, int lane)
-{
-    return (((r >> 3) * 16 + 8 * (lane >> 4) + 2 * (lane & 3)) * 8 + (r & 7)) * 16 + 4 * ((lane >> 2) & 3);
-}
-// the two 4-byte halves land 128 B apart (consecutive K-chunks)
-__device__ __forceinline__ uint2 pack_tile_pair(half2 a, half2 b)
-{
-    uint2 o; o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
-    return o;
-}
-__device__ __forceinline__ void store_tile_pair(uint8_t* p, uint2 o)
-{
-    *reinterpret_cast<uint32_t*>(p) = o.x;
-    *reinterpret_cast<uint32_t*>(p + 128) = o.y;
-}
+// ---- input transform into the tiled activation layout (xt_tile_offset, tc_common.cuh) -------------------------
 template <bool HAD>
 __global__ void __launch_bounds__(128)
 had_tiled_kernel(const half* __restrict__ A, uint8_t* __restrict__ out, const half* __restrict__ suh,
@@ -97,14 +79,6 @@ __host__ __device__ inline TcSmemLayout xt_smem_layout(int K, int b_bytes, int s
     L.total = L.off_bars + 1024;
     L.off_d = L.total;
     return L;
-}
-
-// D[64 x 16] (f32) += A[64 x 16] (f16, registers) * B[16 x 16] (f16, shared memory, K-major)
-__device__ __forceinline__ void wgmma_f16_n16(float (&d)[8], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc)
-{
-    asm volatile("wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, 1, 1, 1, 0;"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc) : "memory");
 }
 
 template <int K, int cb>

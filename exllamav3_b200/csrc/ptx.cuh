@@ -225,6 +225,14 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes
     return d;
 }
 
+// D[64 x 16] (f32) += A[64 x 16] (f16, registers) * B[16 x 16] (f16, shared memory, K-major)
+__device__ __forceinline__ void wgmma_f16_n16(float (&d)[8], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc)
+{
+    asm volatile("wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, 1, 1, 1, 0;"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc) : "memory");
+}
+
 // D[64 x 8] (s32) += A[64 x 32] (u8, registers) * B[32 x 8] (s8, shared memory, K-major)
 __device__ __forceinline__ void wgmma_u8s8_n8(uint32_t (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc)
 {

@@ -105,6 +105,28 @@ __host__ __device__ __forceinline__ int cta_of_unit(int U, int G, int g)
 }
 
 
+#ifdef __CUDACC__
+// ---- input transform into the tiled activation layout ---------------------------------------------------------
+// Tile of one unit: [NT / 8 row groups][16 K-chunks][8 rows][8 fp16], K-chunks 128 B apart, row groups 2048 B apart.  K order:
+// k = 16 kt + 4 j + 2 h + e (kt = 4 r + c) sits in K-chunk 2 (4 r + j) + h at element 2 c + e, i.e. lane l's four values
+// k = 4 l .. 4 l + 3 go to K-chunks 8 (l / 16) + 2 (l % 4) (+1 for the second pair), element pair (l / 4) % 4.
+__device__ __forceinline__ int xt_tile_offset(int r, int lane)
+{
+    return (((r >> 3) * 16 + 8 * (lane >> 4) + 2 * (lane & 3)) * 8 + (r & 7)) * 16 + 4 * ((lane >> 2) & 3);
+}
+// the two 4-byte halves land 128 B apart (consecutive K-chunks)
+__device__ __forceinline__ uint2 pack_tile_pair(half2 a, half2 b)
+{
+    uint2 o; o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
+    return o;
+}
+__device__ __forceinline__ void store_tile_pair(uint8_t* p, uint2 o)
+{
+    *reinterpret_cast<uint32_t*>(p) = o.x;
+    *reinterpret_cast<uint32_t*>(p + 128) = o.y;
+}
+#endif
+
 int get_weight_tmap(const void* B, int k, int n, int K, CUtensorMap* out);
 extern unsigned long long* g_tc_dbg;
 extern int g_tc_knob;

@@ -8,6 +8,7 @@ behaviour (RuntimeError for shape/dtype violations) as the pybind11 bindings the
     had_r_128, hgemm                           bindings.cpp:125,147
     BC_LinearEXL3                              exllamav3_ext/libtorch/linear_bc.h:13-35, linear.cpp:34-71
     exl3_gemv, g_get_cc, g_get_num_sms, exl3_gemm_num_kernel_shapes, exl3_gemm_shape_compat     bindings.cpp:127-131
+    exl3_moe, exl3_moe_max_concurrency         bindings.cpp:209-210
 
 PyTorch is plumbing only here: device memory, the current CUDA stream and the device guard.
 There is no CPU or torch fallback: if the shared library is missing this module fails to import, and every op
@@ -84,6 +85,17 @@ _lib.exl3b_chain_create.argtypes = [ctypes.POINTER(_ChainOp), _i, ctypes.POINTER
 _lib.exl3b_chain_run.argtypes = [_vp, _vp]; _lib.exl3b_chain_run.restype = _i
 _lib.exl3b_chain_destroy.argtypes = [_vp]; _lib.exl3b_chain_destroy.restype = _i
 
+
+class MoePlan(ctypes.Structure):
+    _fields_ = [("passes", ctypes.c_int32), ("chunks", ctypes.c_int32), ("rows", ctypes.c_int32), ("chunk_rows", ctypes.c_int32),
+                ("max_passes", ctypes.c_int32), ("max_chunks", ctypes.c_int32), ("units_gate_up", _i64), ("units_down", _i64)]
+
+
+_lib.exl3b_moe.argtypes = [_vp] * 6 + [_i] * 11 + [_vp] * 9 + [_i] * 6 + [_f, _i]
+_lib.exl3b_moe.restype = _i
+_lib.exl3b_moe_max_concurrency.argtypes = [_i]; _lib.exl3b_moe_max_concurrency.restype = _i
+_lib.exl3b_moe_plan.argtypes = [_vp, _i, _i, _i, _i, _i, ctypes.POINTER(MoePlan), _vp, _vp]; _lib.exl3b_moe_plan.restype = _i
+
 assert _lib.exl3b_abi_version() == 1
 
 EXL3B_TAG_SIMT = 100
@@ -92,6 +104,7 @@ EXL3B_TAG_TC_I8 = 210
 EXL3B_TAG_TC_I8_CHAIN = 220
 EXL3B_TAG_TC_I8_AR = 211
 EXL3B_TAG_TC_I8_ROUTED = 212
+EXL3B_TAG_TC_MOE = 230
 TP_HANDLE_BYTES = 64
 
 lib = _lib      # raw handle for bench.py / tests (symbol export checks)
@@ -454,6 +467,95 @@ def exl3_mgemm(A, B, C, suh, A_had, svh, indices, weights, K: int, force_shape_i
             bszm_in, bszm_out, m, k, n, int(K), _cb(mcg, mul1), int(c_fp32),
             int(min_index), int(max_index), int(num_tokens),
             _ptr(size_n_list), _ptr(c_ptrs), num_c_ptrs, int(force_shape_idx), int(force_num_sms)))
+
+
+def exl3_moe_max_concurrency(device: int) -> int:
+    """Expert groups the reference's fused MoE kernel runs at once: num_sms // 8 (exllamav3_ext/quant/exl3_moe.cu:14-18)."""
+    return _check(_lib.exl3b_moe_max_concurrency(int(device)))
+
+
+def exl3_moe_plan(expert_count, max_tokens: int, num_positions: int, hidden: int, intermediate: int):
+    """Host-only view of the work list the device derives from these counts (include/exl3b200.h): (MoePlan,
+    [(expert, pos0, rows, row0, chunk) per pass], numpy int32 code per position: 128 * pass + row, -1 = not processed)."""
+    import numpy as np
+    c = np.ascontiguousarray(np.asarray(expert_count, dtype=np.int64))
+    E = c.shape[0] - 1
+    args = (c.ctypes.data, E, int(max_tokens), int(num_positions), int(hidden), int(intermediate))
+    out = MoePlan()
+    _check(_lib.exl3b_moe_plan(*args, ctypes.byref(out), None, None))
+    buf = np.zeros(5 * max(out.max_passes, 1), dtype=np.int32)
+    codes = np.zeros(max(int(num_positions), 1), dtype=np.int32)
+    _check(_lib.exl3b_moe_plan(*args, ctypes.byref(out), buf.ctypes.data, codes.ctypes.data))
+    return out, [tuple(int(v) for v in buf[5 * i:5 * i + 5]) for i in range(out.passes)], codes[:int(num_positions)]
+
+
+def exl3_moe(hidden_state, output_state, expert_count, token_sorted, weight_sorted,
+             temp_state_g, temp_state_u, temp_intermediate_g, temp_intermediate_u,
+             act_function: int, K_gate: int, K_up: int, K_down: int,
+             gate_ptrs_trellis, gate_ptrs_suh, gate_ptrs_svh,
+             up_ptrs_trellis, up_ptrs_suh, up_ptrs_svh,
+             down_ptrs_trellis, down_ptrs_suh, down_ptrs_svh,
+             gate_mcg, gate_mul1, up_mcg, up_mul1, down_mcg, down_mul1,
+             act_limit: float, num_active: int) -> None:
+    """
+    Fused routed-expert MLP, exllamav3_ext/quant/exl3_moe.cu:36-200: for every expert with 0 < count <= temp_state_g.size(1)
+    tokens, output_state[t] += w * down(act(gate(x_t)) * up(x_t)) over its positions.  Experts with more tokens, and tokens
+    routed nowhere, are left to the caller: their rows of output_state keep their bits.  Unlike the reference, each token's
+    contributions are added in ascending position order, so the result is deterministic.  The temp buffers are validated as
+    the reference does but not used (the library keeps its own scratch).  num_active = 0 launches nothing.
+    """
+    if num_active == 0:
+        return
+    tabs = (gate_ptrs_trellis, gate_ptrs_suh, gate_ptrs_svh, up_ptrs_trellis, up_ptrs_suh, up_ptrs_svh,
+            down_ptrs_trellis, down_ptrs_suh, down_ptrs_svh)
+    _need_cuda(hidden_state, output_state, expert_count, token_sorted, weight_sorted,
+               temp_state_g, temp_state_u, temp_intermediate_g, temp_intermediate_u, *tabs)
+    _dtype(hidden_state, torch.half, "hidden_state")
+    if hidden_state.dim() != 2:
+        raise RuntimeError("hidden_state: incorrect number of dimensions, must be 2")
+    bsz, hidden = hidden_state.shape
+    _dtype(output_state, torch.float, "output_state")
+    if output_state.shape != hidden_state.shape:
+        raise RuntimeError("output_state and hidden_state have incompatible shapes")
+    _dtype(expert_count, torch.long, "expert_count")
+    if expert_count.dim() != 1:
+        raise RuntimeError("expert_count: incorrect number of dimensions, must be 1")
+    num_experts = expert_count.shape[0] - 1
+    _dtype(token_sorted, torch.long, "token_sorted")
+    if token_sorted.dim() != 1:
+        raise RuntimeError("token_sorted: incorrect number of dimensions, must be 1")
+    _dtype(weight_sorted, torch.half, "weight_sorted")
+    if weight_sorted.shape != token_sorted.shape:
+        raise RuntimeError("token_sorted and weight_sorted have incompatible shapes")
+    for t, name in ((temp_state_g, "temp_state_g"), (temp_state_u, "temp_state_u"),
+                    (temp_intermediate_g, "temp_intermediate_g"), (temp_intermediate_u, "temp_intermediate_u")):
+        _dtype(t, torch.half, name)
+        if t.dim() != 3:
+            raise RuntimeError(f"{name}: incorrect number of dimensions, must be 3")
+    if temp_state_g.shape[2] != hidden or temp_state_u.shape != temp_state_g.shape:
+        raise RuntimeError("temp_state_g / temp_state_u incompatible shapes")
+    if temp_intermediate_u.shape != temp_intermediate_g.shape or temp_intermediate_g.shape[1] != temp_state_g.shape[1]:
+        raise RuntimeError("temp_intermediate_g / temp_intermediate_u incompatible shapes")
+    concurrency, max_tokens, _ = temp_state_g.shape
+    intermediate = temp_intermediate_g.shape[2]
+    for t in tabs:
+        _dtype(t, torch.long, "pointer table")
+        if t.dim() != 1:
+            raise RuntimeError("pointer table: incorrect number of dimensions, must be 1")
+    if gate_ptrs_trellis.shape[0] != num_experts:
+        raise RuntimeError("Number of gate tensors doesn't match num_experts")
+    if any(t.shape != gate_ptrs_trellis.shape for t in tabs):
+        raise RuntimeError("pointer tables have incompatible shapes")
+    for t in (hidden_state, output_state, expert_count, token_sorted, weight_sorted, *tabs):
+        if not t.is_contiguous():
+            raise RuntimeError("exl3_moe: tensors must be contiguous")
+    with torch.cuda.device(hidden_state.device):
+        _check(_lib.exl3b_moe(
+            _stream(hidden_state), _ptr(hidden_state), _ptr(output_state), _ptr(expert_count), _ptr(token_sorted),
+            _ptr(weight_sorted), bsz, hidden, intermediate, num_experts, token_sorted.shape[0], max_tokens, concurrency,
+            int(act_function), int(K_gate), int(K_up), int(K_down), *[_ptr(t) for t in tabs],
+            int(bool(gate_mcg)), int(bool(gate_mul1)), int(bool(up_mcg)), int(bool(up_mul1)),
+            int(bool(down_mcg)), int(bool(down_mul1)), float(act_limit), int(num_active)))
 
 
 def reconstruct_slice(unpacked, packed, K: int, mcg, mul1, n_offset: int) -> None:

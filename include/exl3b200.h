@@ -12,7 +12,8 @@
  *     name ends in `_host`.  `stream` is a `cudaStream_t` passed as `void*` (NULL = legacy default stream).
  *   - the caller owns all buffers.  The library allocates its per-device scratch (split-K partials, tile counters,
  *     transformed-activation buffers for in_features <= 65536) with cudaMalloc ONCE, on the first call on a device, like the
- *     reference's DevCtx (exllamav3_ext/quant/exl3_devctx.cu:24-70); it is never freed, moved or grown afterwards, so a
+ *     reference's DevCtx (exllamav3_ext/quant/exl3_devctx.cu:24-70); exl3b_moe adds its own fixed work area on its first call
+ *     on a device.  Scratch is never freed, moved or grown afterwards, so a
  *     CUDA graph captured over these entry points stays valid, and no entry point allocates or synchronises once the device
  *     context exists (make the first call on a device OUTSIDE stream capture).
  *   - Threading / streams: the scratch is per DEVICE and shared by all streams; launches rotate through 8 scratch slots, so
@@ -58,6 +59,7 @@ enum exl3b_status
 #define EXL3B_TAG_TC_I8_ROUTED 212 /* routed / weighted exl3b_mgemm (MoE decode) on the kind::i8 kernel: mul1, m <= 4 (auto) */
 #define EXL3B_TAG_TC_I8_CHAIN 220 /* persistent multi-GEMM kernel (exl3b_chain_*; exl3b_gemm when forced): mul1, m <= 4 */
 #define EXL3B_TAG_TC_I8_AR 211 /* the same kernel with the tensor-parallel sum fused into its epilogue (exl3b_gemm_allreduce) */
+#define EXL3B_TAG_TC_MOE 230   /* fused routed-expert MLP (exl3b_moe) on the exact wgmma decode-GEMM                          */
 
 int exl3b_abi_version(void);
 
@@ -201,6 +203,52 @@ int exl3b_chain_walk(const struct exl3b_chain_op* ops, int n_ops, int num_sms, i
 int exl3b_chain_create(const struct exl3b_chain_op* ops, int n_ops, void** chain);
 int exl3b_chain_run(void* stream, void* chain);
 int exl3b_chain_destroy(void* chain);
+
+/*
+ * exl3b_moe -- replaces ext.exl3_moe (exllamav3_ext/bindings.cpp:209, exllamav3_ext/quant/exl3_moe.cu): the routed experts'
+ * gated MLP of a mixture-of-experts block in one call.  E = num_experts experts; expert e owns positions [s_e, s_e + c_e) of
+ * token_sorted / weight_sorted, s_e = sum of expert_count[0..e), c_e = expert_count[e] (expert_count has E + 1 entries, the
+ * last one is ignored).  Experts with 0 < c_e <= max_tokens are processed; for each of their positions j, t = token_sorted[j]:
+ *   g = gate_e(x_t), u = up_e(x_t)            as exl3b_gemm with fp16 output (act_function 2: no gate GEMM)
+ *   h = fp16(act(g) * u)                      act 0 = SiLU, 1 = tanh-GELU, 2 = ReLU^2 of u (h = relu(u) * u)
+ *                                             act_limit != 0: u clamped to [-L, L], act(g) <= L
+ *   output_state[t] += weight_sorted[j] * down_e(h)     fp32, added in ascending j: the result is deterministic
+ * Other rows of output_state keep their bits.
+ *   hidden_state (bsz, hidden) fp16 (8-byte aligned), output_state (bsz, hidden) fp32 (16-byte aligned), expert_count (E + 1)
+ *   int64, token_sorted and weight_sorted (num_positions) int64 / fp16; the nine tables: E device addresses each; cb 1 = mcg or
+ *   2 = mul1 for all three; hidden % 128 == intermediate % 128 == 0, K_* in 1..8, E <= 2048, concurrency * 8 <= num_sms,
+ *   num_positions and bsz <= 2^20.  The caller's temp buffers are not needed.  The first call on a device allocates the
+ *   operator's fixed work area (about 256 MB: the work list of up to 2^20 positions and a 240 MB row region); it is never
+ *   grown, so make that first call outside stream capture, like the first call of any entry point.  Calls whose processed rows
+ *   do not fit the row region at once run in several chunks of passes, with the same result bit for bit.
+ *   num_active = 0: nothing is launched (EXL3B_TAG_NOP).  Returns EXL3B_TAG_TC_MOE.
+ * exl3b_moe_max_concurrency(device) = num_sms / 8, as the reference (callers size their temp buffers from it).
+ * exl3b_moe_plan: host-only introspection of the work list the route kernel derives on the device from the same counts, by
+ * the same code: the passes (up to 128 consecutive positions of one processed expert, rows padded to 16) packed in order into
+ * chunks of at most chunk_rows rows, written as int32 (expert, pos0, rows, row0, chunk) quintuples to passes_out (NULL = not
+ * written; room for max_passes), and every position's code (128 * pass + row in pass, -1 = not processed) to pos_code_out
+ * (num_positions entries, or NULL).  units_*: work items (pass, 128-column strip) of the gate / up and the down GEMMs.
+ */
+struct exl3b_moe_plan
+{
+    int32_t passes, chunks;          /* passes and chunks of the call                                        */
+    int32_t rows, chunk_rows;        /* most rows any chunk uses, rows one chunk may hold                      */
+    int32_t max_passes, max_chunks;  /* the launcher's bounds from sizes alone (grids, chunk launches)         */
+    int64_t units_gate_up, units_down;
+};
+int exl3b_moe(void* stream,
+              const void* hidden_state, void* output_state,
+              const int64_t* expert_count, const int64_t* token_sorted, const void* weight_sorted,
+              int bsz, int hidden, int intermediate, int num_experts, int num_positions, int max_tokens, int concurrency,
+              int act_function, int K_gate, int K_up, int K_down,
+              const uint64_t* gate_trellis, const uint64_t* gate_suh, const uint64_t* gate_svh,
+              const uint64_t* up_trellis, const uint64_t* up_suh, const uint64_t* up_svh,
+              const uint64_t* down_trellis, const uint64_t* down_suh, const uint64_t* down_svh,
+              int gate_mcg, int gate_mul1, int up_mcg, int up_mul1, int down_mcg, int down_mul1,
+              float act_limit, int num_active);
+int exl3b_moe_max_concurrency(int device);
+int exl3b_moe_plan(const int64_t* expert_count_host, int num_experts, int max_tokens, int num_positions, int hidden,
+                   int intermediate, struct exl3b_moe_plan* out, int32_t* passes_out, int32_t* pos_code_out);
 
 /*
  * exl3b_reconstruct -- replaces ext.reconstruct / ext.reconstruct_slice (exllamav3_ext/bindings.cpp:122-123,
