@@ -471,6 +471,27 @@ int exl3b_moe(void* stream, const void* hidden_state, void* output_state,
     return launch_moe((cudaStream_t) stream, ctx, a);
 }
 
+int exl3b_quantize_tiles(void* stream, const void* in, void* out_tiles, void* out_idx, int64_t num_tiles, int K, int cb)
+{
+    int r = check_kcb(K, cb); if (r) return r;
+    EXL3B_CHECK(num_tiles >= 0, EXL3B_ERR_SHAPE, "quantize_tiles: negative number of tiles");
+    if (num_tiles == 0) return 0;
+    EXL3B_CHECK(in && out_tiles && out_idx, EXL3B_ERR_ARG, "quantize_tiles: null tensor");
+    DevCtx* ctx; r = get_ctx(&ctx); if (r) return r;
+    return launch_quantize_tiles((cudaStream_t) stream, ctx, (const float*) in, (float*) out_tiles, (uint16_t*) out_idx,
+                                 num_tiles, K, cb);
+}
+
+int exl3b_pack_trellis(void* stream, void* packed, const void* unpacked, int64_t num_tiles, int K)
+{
+    EXL3B_CHECK(K >= 1 && K <= 8, EXL3B_ERR_ARG, "K must be 1..8, got %d", K);
+    EXL3B_CHECK(num_tiles >= 0, EXL3B_ERR_SHAPE, "pack_trellis: negative number of tiles");
+    if (num_tiles == 0) return 0;
+    EXL3B_CHECK(packed && unpacked, EXL3B_ERR_ARG, "pack_trellis: null tensor");
+    DevCtx* ctx; int r = get_ctx(&ctx); if (r) return r;
+    return launch_pack_trellis((cudaStream_t) stream, (uint16_t*) packed, (const uint16_t*) unpacked, num_tiles, K);
+}
+
 int exl3b_hgemm(void* stream, const void* a, const void* b, void* c, int m, int k, int n, int c_fp32,
                 int64_t c_stride)
 {

@@ -190,6 +190,11 @@ int launch_moe(cudaStream_t stream, DevCtx* ctx, const MoeArgs& a);
 int moe_plan_host(const int64_t* count, int E, int T, int N, int hidden, int inter, struct exl3b_moe_plan* out, int32_t* passes_out,
                   int32_t* pos_code_out);
 
+// trellis encoder (encode.cu): tail-biting Viterbi per 256-value tile, and the K-bit packer
+int launch_quantize_tiles(cudaStream_t stream, DevCtx* ctx, const float* in, float* out_values, uint16_t* out_states,
+                          int64_t num_tiles, int K, int cb);
+int launch_pack_trellis(cudaStream_t stream, uint16_t* packed, const uint16_t* unpacked, int64_t num_tiles, int K);
+
 // ---- (K, cb) template dispatch ---------------------------------------------------------------------------------
 #define EXL3B_DISPATCH_K_CB(FN, K, cb, ...)                                                        \
     do { switch ((cb) * 8 + (K) - 1) {                                                             \

@@ -9,6 +9,7 @@ behaviour (RuntimeError for shape/dtype violations) as the pybind11 bindings the
     BC_LinearEXL3                              exllamav3_ext/libtorch/linear_bc.h:13-35, linear.cpp:34-71
     exl3_gemv, g_get_cc, g_get_num_sms, exl3_gemm_num_kernel_shapes, exl3_gemm_shape_compat     bindings.cpp:127-131
     exl3_moe, exl3_moe_max_concurrency         bindings.cpp:209-210
+    quantize_tiles, pack_trellis               bindings.cpp:116,119 (the converter's trellis encoder)
 
 PyTorch is plumbing only here: device memory, the current CUDA stream and the device guard.
 There is no CPU or torch fallback: if the shared library is missing this module fails to import, and every op
@@ -95,6 +96,8 @@ _lib.exl3b_moe.argtypes = [_vp] * 6 + [_i] * 11 + [_vp] * 9 + [_i] * 6 + [_f, _i
 _lib.exl3b_moe.restype = _i
 _lib.exl3b_moe_max_concurrency.argtypes = [_i]; _lib.exl3b_moe_max_concurrency.restype = _i
 _lib.exl3b_moe_plan.argtypes = [_vp, _i, _i, _i, _i, _i, ctypes.POINTER(MoePlan), _vp, _vp]; _lib.exl3b_moe_plan.restype = _i
+_lib.exl3b_quantize_tiles.argtypes = [_vp] * 4 + [_i64, _i, _i]; _lib.exl3b_quantize_tiles.restype = _i
+_lib.exl3b_pack_trellis.argtypes = [_vp] * 3 + [_i64, _i]; _lib.exl3b_pack_trellis.restype = _i
 
 assert _lib.exl3b_abi_version() == 1
 
@@ -716,3 +719,74 @@ class BC_LinearEXL3:
             return y
         self.run(x.view(-1, x.shape[-1]), y.view(-1, out_features))
         return y
+
+
+# ---- trellis encoder (the converter's two GPU bindings, modules/quant/exl3_lib/quantize.py) ---------------------------------
+
+def _same_cuda_contiguous(op: str, *ts):
+    _need_cuda(*ts)
+    dev = ts[0].device
+    for t in ts:
+        if t.device != dev:
+            raise RuntimeError(f"{op}: all tensors must be on the same device")
+        if not t.is_contiguous():
+            raise RuntimeError(f"{op}: all tensors must be contiguous")
+
+
+def quantize_tiles(input_tiles, output_tiles, output_indices, temp_costs, temp_edges, K: int, mcg, mul1) -> None:
+    """
+    Trellis-quantize tiles: row i of input_tiles (N, 256) fp32 holds one tile in trellis position order; output_indices
+    (int16) receives the tail-biting state sequence of least squared error and output_tiles (fp32) its codebook values.
+    exllamav3_ext/quant/quantize.cu:23-92.  The temp buffers are validated as the reference does and otherwise unused:
+    the kernel keeps its backpointers as K-bit choices in a fixed per-device scratch (include/exl3b200.h).
+    """
+    if input_tiles.dim() != 2:
+        raise RuntimeError("input_tiles: incorrect number of dimensions, must be 2")
+    if input_tiles.shape[1] != 256:
+        raise RuntimeError("input_tiles: incorrect size of dimension 1, must be 256")
+    if tuple(output_indices.shape) != tuple(input_tiles.shape) or tuple(output_tiles.shape) != tuple(input_tiles.shape):
+        raise RuntimeError("input_tiles, output_tiles and output_indices must have the same shape")
+    _dtype(input_tiles, torch.float, "input_tiles")
+    _dtype(output_tiles, torch.float, "output_tiles")
+    _dtype(output_indices, torch.int16, "output_indices")
+    K = int(K)
+    if not 1 <= K <= 8:
+        raise RuntimeError("quantize_tiles K must be in range 1..8")
+    cb = _cb(mcg, mul1)
+    num_tiles = input_tiles.shape[0]
+    if num_tiles == 0:
+        return
+    edges = 65536 >> K
+    _dtype(temp_costs, torch.half, "temp_costs")
+    if temp_costs.dim() != 3 or temp_costs.shape[1] != 2 or temp_costs.shape[2] != edges:
+        raise RuntimeError(f"temp_costs must have shape (B, 2, {edges})")
+    _dtype(temp_edges, torch.int16, "temp_edges")
+    if temp_edges.dim() != 3 or temp_edges.shape[1] != 256 or temp_edges.shape[2] != edges:
+        raise RuntimeError(f"temp_edges must have shape (B, 256, {edges})")
+    _same_cuda_contiguous("quantize_tiles", input_tiles, output_tiles, output_indices, temp_costs, temp_edges)
+    with torch.cuda.device(input_tiles.device):
+        _check(_lib.exl3b_quantize_tiles(_stream(input_tiles), _ptr(input_tiles), _ptr(output_tiles), _ptr(output_indices),
+                                         num_tiles, K, cb))
+
+
+def pack_trellis(packed, unpacked, K: int) -> None:
+    """unpacked (a, b, 256) int16 states -> packed (a, b, 16K) int16 trellis.  exllamav3_ext/quant/pack.cu:61-86."""
+    K = int(K)
+    if not 1 <= K <= 8:
+        raise RuntimeError("pack_trellis K must be in range 1..8")
+    if packed.dim() != 3 or unpacked.dim() != 3:
+        raise RuntimeError("packed and unpacked: incorrect number of dimensions, must be 3")
+    if packed.shape[0] != unpacked.shape[0] or packed.shape[1] != unpacked.shape[1]:
+        raise RuntimeError("packed and unpacked have incompatible shapes")
+    if unpacked.shape[2] != 256:
+        raise RuntimeError("unpacked: incorrect size of dimension 2, must be 256")
+    if packed.shape[2] != 16 * K:
+        raise RuntimeError(f"packed: incorrect size of dimension 2, must be {16 * K}")
+    _dtype(packed, torch.int16, "packed")
+    _dtype(unpacked, torch.int16, "unpacked")
+    num_tiles = unpacked.shape[0] * unpacked.shape[1]
+    if num_tiles == 0:
+        return
+    _same_cuda_contiguous("pack_trellis", packed, unpacked)
+    with torch.cuda.device(unpacked.device):
+        _check(_lib.exl3b_pack_trellis(_stream(unpacked), _ptr(packed), _ptr(unpacked), num_tiles, K))

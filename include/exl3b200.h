@@ -12,8 +12,8 @@
  *     name ends in `_host`.  `stream` is a `cudaStream_t` passed as `void*` (NULL = legacy default stream).
  *   - the caller owns all buffers.  The library allocates its per-device scratch (split-K partials, tile counters,
  *     transformed-activation buffers for in_features <= 65536) with cudaMalloc ONCE, on the first call on a device, like the
- *     reference's DevCtx (exllamav3_ext/quant/exl3_devctx.cu:24-70); exl3b_moe adds its own fixed work area on its first call
- *     on a device.  Scratch is never freed, moved or grown afterwards, so a
+ *     reference's DevCtx (exllamav3_ext/quant/exl3_devctx.cu:24-70); exl3b_moe and exl3b_quantize_tiles add their own fixed work
+ *     areas on their first call on a device.  Scratch is never freed, moved or grown afterwards, so a
  *     CUDA graph captured over these entry points stays valid, and no entry point allocates or synchronises once the device
  *     context exists (make the first call on a device OUTSIDE stream capture).
  *   - Threading / streams: the scratch is per DEVICE and shared by all streams; launches rotate through 8 scratch slots, so
@@ -336,6 +336,24 @@ int exl3b_gemm_allreduce_check(int m, int k, int n, int K, int cb, int world, in
 int exl3b_tp_debug_inject(void* stream, int src_rank, const void* partial, int64_t count);
 int exl3b_tp_debug_peek(int buffer_rank, int slot, int src_rank, void* host_out, int64_t count);
 int64_t exl3b_tp_debug_epoch(void);
+
+/*
+ * ---- trellis encoder (conversion) ---------------------------------------------------------------------------------------
+ *
+ * exl3b_quantize_tiles -- replaces ext.quantize_tiles (exllamav3_ext/bindings.cpp:116, quant/quantize.cu): for each of
+ * num_tiles rows of 256 fp32 values `in` (one 16x16 tile in trellis position order), the tail-biting state sequence
+ * s[0..255] of minimum squared error against the codebook cb, found by Viterbi with fp32 path costs.  Writes the states
+ * (uint16, num_tiles x 256) to out_idx and their codebook values as fp32 to out_tiles.  The wrap overlap s[0] >> K is
+ * chosen like the reference does (best unconstrained path started at position 128); the sequence is the exact minimum
+ * for that overlap.  Deterministic; a tile's result does not depend on the other tiles of the call.  The first call on
+ * a device allocates a fixed backpointer scratch of 2 MB per SM (make it outside stream capture).
+ *
+ * exl3b_pack_trellis -- replaces ext.pack_trellis (bindings.cpp:119, quant/pack.cu:9-57): unpacked (num_tiles x 256
+ * uint16 states) -> packed (num_tiles x 16K uint16), the low K bits of each state MSB first, 16-bit words swapped
+ * pairwise per 32-bit word: the trellis layout every GEMM entry point reads.
+ */
+int exl3b_quantize_tiles(void* stream, const void* in, void* out_tiles, void* out_idx, int64_t num_tiles, int K, int cb);
+int exl3b_pack_trellis(void* stream, void* packed, const void* unpacked, int64_t num_tiles, int K);
 
 /* Count of kernels launched by this library in this process (for bench.py's gpu_launches claim). */
 int64_t exl3b_launch_count(void);
