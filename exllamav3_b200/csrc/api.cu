@@ -99,7 +99,7 @@ int ensure_xh_tiled(DevCtx* ctx, size_t bytes_per_slot)
 
 }  // namespace exl3b
 
-namespace exl3b { void tc_set_debug_buffer(unsigned long long* d); void tc_set_knob(int k); }
+namespace exl3b { void tc_set_debug_buffer(unsigned long long* d); }
 using namespace exl3b;
 
 extern "C" {
@@ -114,7 +114,6 @@ int exl3b_set_gemm_path(int tag) { return g_force_path.exchange(tag); }
 
 // bring-up aid (not in the public header): per-CTA %globaltimer stamps of the tensor-core kernels, 16 x u64 per CTA
 void exl3b_debug_tc_timeline(void* dev_buf) { exl3b::tc_set_debug_buffer((unsigned long long*) dev_buf); }
-void exl3b_debug_tc_knob(int knob) { exl3b::tc_set_knob(knob); }
 void exl3b_debug_reconstruct_had(int mode) { exl3b::reconstruct_had_set_mode(mode); }
 
 int exl3b_num_sms(int device)

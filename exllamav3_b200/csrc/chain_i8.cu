@@ -24,27 +24,16 @@
 //
 // Roles (768 threads): warp 0 TMA producer, warp 1 idle, warps 2-3 activation / digit warps, warps 4-19 decode + MMA (two
 // groups of two warpgroups), warps 20-23 epilogue; accumulators reach the epilogue through two shared-memory buffers.
-#include "tc_common.cuh"
-#include "i8_math.cuh"
+#include "i8_pipeline.cuh"
 #include <mutex>
 #include <vector>
 
 namespace exl3b {
 
-using namespace ptx;
-
-constexpr int CH_THREADS = 768;
-constexpr int CH_XF_WARP0 = 2, CH_XF_WARPS = 2;
-constexpr int CH_DEC_WARP0 = 4, CH_DEC_WARPS = 16, CH_DEC_GROUPS = 2;
-constexpr int CH_EPI_WARP0 = 20;
 constexpr int CH_MR = 4;
-constexpr int CH_B_BYTES = 4096, CH_B_STAGE = 4096 + 64;               // digit tile + per-row digit sums
-constexpr int CH_SUB_UNITS = 96;                                       // int32 accumulator safety (see I8_SUB_UNITS)
-constexpr int CH_MAX_STAGES = 16;
+constexpr int CH_XF_WARPS = TC_DEC_WARP0 - TC_XF_WARP0;
 constexpr int CH_MAX_INLINE = 4;
 constexpr int CH_SCALE_SLOTS = 32;
-constexpr uint32_t CH_SENTINEL = 0xffffffffu;
-constexpr int CH_CACHE_MAX = 64 * 1024;
 
 struct ChainOp
 {
@@ -77,20 +66,17 @@ struct ChainParams
     CUtensorMap tmaps_inline[CH_MAX_INLINE];
 };
 
-// accumulator hand-off decode groups -> epilogue: [2 buffers][2 groups][128 columns][2 CH_MR] int32, then [2][2][8] digit sums
-constexpr int CH_D_BYTES = 2 * 2 * 128 * 2 * CH_MR * 4 + 2 * 2 * 8 * 4;
-
 struct ChainSmem { int off_b, off_tile, off_bars, off_d, off_cache, off_suh, total; };
 
 __host__ __device__ inline ChainSmem chain_smem(int S, int w_bytes, int cache_bytes, int suh_bytes)
 {
     ChainSmem L;
     L.off_b = S * w_bytes;
-    L.off_tile = L.off_b + S * CH_B_STAGE;
+    L.off_tile = L.off_b + S * i8_b_stage(CH_MR);
     L.off_tile = (L.off_tile + 127) & ~127;
     L.off_bars = L.off_tile + CH_MR * 128 * 4;
     L.off_d = L.off_bars + 2048;
-    L.off_cache = L.off_d + CH_D_BYTES;
+    L.off_cache = L.off_d + i8_d_bytes(CH_MR);
     L.off_suh = L.off_cache + cache_bytes;
     L.total = L.off_suh + suh_bytes;
     return L;
@@ -152,11 +138,11 @@ struct Cursor
             start_run();
         }
     }
-    // bounds of the accumulation chunk (<= CH_SUB_UNITS units of the run) that holds the current unit
+    // bounds of the accumulation chunk (<= I8_SUB_UNITS units of the run) that holds the current unit
     __host__ __device__ __forceinline__ void sub_bounds(int& sb, int& se) const
     {
-        sb = run_begin + (seq - run_begin) / CH_SUB_UNITS * CH_SUB_UNITS;
-        se = sb + CH_SUB_UNITS < run_end ? sb + CH_SUB_UNITS : run_end;
+        sb = run_begin + (seq - run_begin) / I8_SUB_UNITS * I8_SUB_UNITS;
+        se = sb + I8_SUB_UNITS < run_end ? sb + I8_SUB_UNITS : run_end;
     }
 };
 
@@ -171,13 +157,13 @@ struct ChainCtx
     unsigned long long* dbg;
     int trace_seq;            // bring-up: the unit (CTA-local index) whose steps are stamped
     __device__ __forceinline__ uint32_t W_FULL(int s) const { return bar0 + 8u * s; }
-    __device__ __forceinline__ uint32_t W_EMPTY(int s) const { return bar0 + 8u * (CH_MAX_STAGES + s); }
-    __device__ __forceinline__ uint32_t X_FULL(int s) const { return bar0 + 8u * (2 * CH_MAX_STAGES + s); }
-    __device__ __forceinline__ uint32_t D_FULL(int b) const { return bar0 + 8u * (3 * CH_MAX_STAGES + 8 + b); }
-    __device__ __forceinline__ uint32_t D_EMPTY(int b) const { return bar0 + 8u * (3 * CH_MAX_STAGES + 10 + b); }
-    __device__ __forceinline__ uint32_t IN_BAR() const { return bar0 + 8u * (3 * CH_MAX_STAGES + 12); }
+    __device__ __forceinline__ uint32_t W_EMPTY(int s) const { return bar0 + 8u * (TC_MAX_STAGES + s); }
+    __device__ __forceinline__ uint32_t X_FULL(int s) const { return bar0 + 8u * (2 * TC_MAX_STAGES + s); }
+    __device__ __forceinline__ uint32_t D_FULL(int b) const { return bar0 + 8u * (3 * TC_MAX_STAGES + 8 + b); }
+    __device__ __forceinline__ uint32_t D_EMPTY(int b) const { return bar0 + 8u * (3 * TC_MAX_STAGES + 10 + b); }
+    __device__ __forceinline__ uint32_t IN_BAR() const { return bar0 + 8u * (3 * TC_MAX_STAGES + 12); }
 };
-constexpr int CH_NUM_BARS = 3 * CH_MAX_STAGES + 13;                    // 61 barriers
+constexpr int CH_NUM_BARS = 3 * TC_MAX_STAGES + 13;                    // 61 barriers
 
 #ifdef EXL3B_TC_DEBUG
 #define CH_STAMP(cond, slot) do { if ((cond) && cx.dbg) { unsigned long long t__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t__) :: "memory"); cx.dbg[blockIdx.x * 64 + (slot)] = t__; } } while (0)
@@ -185,72 +171,30 @@ constexpr int CH_NUM_BARS = 3 * CH_MAX_STAGES + 13;                    // 61 bar
 #define CH_STAMP(cond, slot) do { } while (0)
 #endif
 
-// One unit (128 k x 128 n weights) of a decode warpgroup: the pipeline of gemm_tc_i8_body.cuh -- weight words from the ring
-// stage, the warp's tile column of k-tiles c and 4 + c decoded straight into wgmma A fragments, 16 MMAs into acc.
+// One unit of a decode warp: wait for the ring stage's weights and digits, then i8_unit_mma.
 template <int K>
 __device__ __forceinline__ void group_unit(const ChainCtx& cx, int tl, int lane, int s, int sph, int m, uint32_t (&acc)[CH_MR], int& tsum,
                                            [[maybe_unused]] bool trace)
 {
-    const int chunk = lane >> 2, c = lane & 3;
+    const int c = lane & 3;
     [[maybe_unused]] const bool tr = trace && tl == 0 && lane == 0;
     CH_STAMP(tr, 0);
     mbar_wait<32>(cx.W_FULL(s), sph);
     CH_STAMP(tr, 1);
-    const uint32_t* wst = reinterpret_cast<const uint32_t*>(cx.smem + s * cx.w_bytes);
-    uint32_t w[2][K + 1];
-    #pragma unroll
-    for (int r = 0; r < 2; ++r) load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, w[r]);
     mbar_wait(cx.X_FULL(s), sph);                                      // the unit's activation digits
     CH_STAMP(tr, 2);
-    if (c < m) tsum += *reinterpret_cast<const int*>(cx.smem + cx.L.off_b + s * CH_B_STAGE + CH_B_BYTES + 4 * c);
-    const uint64_t desc_s = smem_desc(smem_u32(cx.smem + cx.L.off_b + s * CH_B_STAGE), 128, 4096, 0);
-    #pragma unroll
-    for (int r = 0; r < 2; ++r)
-    {
-        uint32_t o0[16], o1[16];
-        decode16_i8<K, 0>(w[r], o0);
-        decode16_i8<K, 1>(w[r], o1);
-        #pragma unroll
-        for (int i = 0; i < CH_MR; ++i) reg_fence(acc[i]);
-        wgmma_fence();
-        #pragma unroll
-        for (int j = 0; j < 8; ++j)
-            wgmma_u8s8_n8(acc, o0[2 * j], o1[2 * j], o0[2 * j + 1], o1[2 * j + 1], desc_s + (uint64_t) (16 * (8 * r + j)));
-        wgmma_commit();
-        wgmma_wait<0>();
-        #pragma unroll
-        for (int i = 0; i < 16; ++i) { reg_fence(o0[i]); reg_fence(o1[i]); }
-        #pragma unroll
-        for (int i = 0; i < CH_MR; ++i) reg_fence(acc[i]);
-    }
+    const uint8_t* b = cx.smem + cx.L.off_b + s * i8_b_stage(CH_MR);
+    if (c < m) tsum += *reinterpret_cast<const int*>(b + i8_b_bytes(CH_MR) + 4 * c);
+    i8_unit_mma<K, CH_MR>(reinterpret_cast<const uint32_t*>(cx.smem + s * cx.w_bytes), smem_desc(smem_u32(b), 128, 4096, 0), tl, lane, acc);
     CH_STAMP(tr, 3);
     __syncwarp();
     if (lane == 0) mbar_arrive(cx.W_EMPTY(s));
 }
 
-__device__ __forceinline__ void ch_watchdog(uint32_t& polls, unsigned long long& t0, const char* what, int a, int b)
-{
-    if ((++polls & 255u) == 0)
-    {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        if (t0 == 0) t0 = t;
-        else if (t - t0 > 4000000000ull)
-        {
-#ifdef EXL3B_TC_DEBUG
-            printf("exl3b chain: %s timeout (block %d, %d, %d)\n", what, blockIdx.x, a, b);
-#else
-            (void) what; (void) a; (void) b;
-#endif
-            __trap();
-        }
-    }
-}
-
 // KSEL = 0: ops of any bitrate (a switch per unit); KSEL = 1..8: every op of the chain has K = KSEL (smaller code: the
 // instruction footprint of all concurrently running roles matters on a kernel this size)
 template <int KSEL>
-__global__ void __launch_bounds__(CH_THREADS, 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 chain_i8_kernel(const __grid_constant__ ChainParams p)
 {
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -269,7 +213,7 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
     unsigned int* s_norm2 = reinterpret_cast<unsigned int*>(misc + 4);                                       // [MR] float bits
     float* s_scale = reinterpret_cast<float*>(misc + 8 + 8);                                                 // [CH_SCALE_SLOTS][MR]
     int32_t* s_d = reinterpret_cast<int32_t*>(smem + cx.L.off_d);                                            // [dbuf][group][128][2 MR]
-    int* s_dt = reinterpret_cast<int*>(smem + cx.L.off_d + CH_D_BYTES - 2 * 2 * 8 * 4);                     // [dbuf][group][8]
+    int* s_dt = reinterpret_cast<int*>(smem + cx.L.off_d + i8_d_bytes(CH_MR) - 2 * 2 * 8 * 4);              // [dbuf][group][8]
     half* cache = reinterpret_cast<half*>(smem + cx.L.off_cache);
     half* suh_s = reinterpret_cast<half*>(smem + cx.L.off_suh);
 
@@ -279,10 +223,10 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
         for (int i = lane; i < CH_NUM_BARS; i += 32)
         {
             int cnt = 1;
-            if (i >= CH_MAX_STAGES && i < 2 * CH_MAX_STAGES) cnt = CH_DEC_WARPS / CH_DEC_GROUPS;         // W_EMPTY: the group's warps, after their MMAs
-            else if (i >= 3 * CH_MAX_STAGES + 8 && i < 3 * CH_MAX_STAGES + 10) cnt = CH_DEC_WARPS;         // D_FULL: every decode warp
-            else if (i >= 3 * CH_MAX_STAGES + 10 && i < 3 * CH_MAX_STAGES + 12) cnt = 4;                 // D_EMPTY: the 4 epilogue warps
-            else if (i == 3 * CH_MAX_STAGES + 12) cnt = 2;                                               // IN_BAR: suh copy + input copy
+            if (i >= TC_MAX_STAGES && i < 2 * TC_MAX_STAGES) cnt = TC_DEC_WARPS / I8_DEC_GROUPS;         // W_EMPTY: the group's warps, after their MMAs
+            else if (i >= 3 * TC_MAX_STAGES + 8 && i < 3 * TC_MAX_STAGES + 10) cnt = TC_DEC_WARPS;         // D_FULL: every decode warp
+            else if (i >= 3 * TC_MAX_STAGES + 10 && i < 3 * TC_MAX_STAGES + 12) cnt = 4;                 // D_EMPTY: the 4 epilogue warps
+            else if (i == 3 * TC_MAX_STAGES + 12) cnt = 2;                                               // IN_BAR: suh copy + input copy
             mbar_init(cx.bar0 + 8u * i, cnt);
         }
         fence_barrier_init();
@@ -318,10 +262,10 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
         }
         __syncwarp();
     }
-    else if (warp >= CH_XF_WARP0 && warp < CH_DEC_WARP0)
+    else if (warp >= TC_XF_WARP0 && warp < TC_DEC_WARP0)
     {
         // =========================== activation warps: scale pass per op, digits per unit ===========================
-        const int xw = warp - CH_XF_WARP0;
+        const int xw = warp - TC_XF_WARP0;
         auto xf_bar = [] { asm volatile("bar.sync 2, %0;" :: "n"(CH_XF_WARPS * 32) : "memory"); };
         pdl_wait();                                                   // external inputs come from the previous kernel
         Cursor c; c.init(ops, stages, p.n_stages, cta, G);
@@ -342,11 +286,11 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                     o.A = g.A; o.A2 = g.A2; o.suh = g.suh; o.m = g.m; o.k = g.k; o.KB = g.KB; o.in_mode = g.in_mode;
                     o.cached = g.cached; o.suh_cached = g.suh_cached; o.stage = g.stage;
                 }
-                CH_STAMP(warp == CH_XF_WARP0 && lane == 0 && c.seq == 0, 59);
+                CH_STAMP(warp == TC_XF_WARP0 && lane == 0 && c.seq == 0, 59);
                 const bool bulk_x = o.in_mode == 0 && o.cached;       // input rows by one bulk copy straight into the cache
                 const bool bulk_s = o.suh != nullptr && o.suh_cached;
                 xf_bar();                                             // previous op's cache / suh no longer needed by any digit warp
-                if (warp == CH_XF_WARP0)
+                if (warp == TC_XF_WARP0)
                 {
                     if (lane < CH_MR) s_norm2[lane] = 0u;
                     // suh does not depend on the previous stage: its copy is in flight while we wait for the stage
@@ -369,12 +313,12 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                     {
                         const unsigned int want = (unsigned int) stages[o.stage - 1].strips_total;
                         uint32_t polls = 0; unsigned long long t0 = 0;
-                        while (ld_acquire_gpu_u32(p.ctr + (o.stage - 1)) < want) { __nanosleep(32); ch_watchdog(polls, t0, "stage wait", o.stage, 0); }
+                        while (ld_acquire_gpu_u32(p.ctr + (o.stage - 1)) < want) { __nanosleep(32); poll_watchdog<255u>(polls, t0, "chain stage wait", o.stage, 0); }
                     }
                     __syncwarp();
                     waited = o.stage;
                 }
-                if (warp == CH_XF_WARP0)
+                if (warp == TC_XF_WARP0)
                 {
                     if (elect_one())
                     {
@@ -479,7 +423,7 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                     // arrive the MMA side observes, the scale the epilogue reads later is ordered before it
                     if (lane == r) s_scale[(cur_op % CH_SCALE_SLOTS) * CH_MR + r] = i8_over_qmax(bnd);
                 }
-                CH_STAMP(warp == CH_XF_WARP0 && lane == 0 && c.seq == 0, 60);
+                CH_STAMP(warp == TC_XF_WARP0 && lane == 0 && c.seq == 0, 60);
             }
             if (turn == xw)
             {
@@ -487,74 +431,36 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                 CH_STAMP(c.seq == cx.trace_seq && lane == 0, 56);
                 mbar_wait<64>(cx.W_EMPTY(s), ph ^ 1);
                 CH_STAMP(c.seq == cx.trace_seq && lane == 0, 57);
-                uint8_t* dst = smem + cx.L.off_b + s * CH_B_STAGE;
-                int qsum[CH_MR];
-                #pragma unroll
-                for (int r = 0; r < CH_MR; ++r)
+                i8_write_digit_tile<CH_MR>(smem + cx.L.off_b + s * i8_b_stage(CH_MR), inv_scale, o.m, lane, cx.X_FULL(s),
+                                           [&](int r, float (&v)[4])
                 {
-                    qsum[r] = 0;
-                    if (r < o.m)
+                    half2 a, b;
+                    if (o.cached)
                     {
-                        half2 a, b;
-                        if (o.cached)
-                        {
-                            const uint2 raw = *reinterpret_cast<const uint2*>(cache + (size_t) r * o.k + c.kb * 128 + lane * 4);
-                            a = *reinterpret_cast<const half2*>(&raw.x); b = *reinterpret_cast<const half2*>(&raw.y);
-                        }
-                        else
-                        {
-                            // rows too long for the cache: recompute the block (plain fp16 input only, checked on the host)
-                            const uint2 raw = __ldcg(reinterpret_cast<const uint2*>(reinterpret_cast<const half*>(o.A) + (size_t) r * o.k + c.kb * 128 + lane * 4));
-                            a = *reinterpret_cast<const half2*>(&raw.x); b = *reinterpret_cast<const half2*>(&raw.y);
-                            if (o.suh)
-                            {
-                                const uint2 scb = *reinterpret_cast<const uint2*>(o.suh + c.kb * 128 + lane * 4);
-                                a = __hmul2(a, *reinterpret_cast<const half2*>(&scb.x));
-                                b = __hmul2(b, *reinterpret_cast<const half2*>(&scb.y));
-                            }
-                        }
-                        float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
+                        const uint2 raw = *reinterpret_cast<const uint2*>(cache + (size_t) r * o.k + c.kb * 128 + lane * 4);
+                        a = *reinterpret_cast<const half2*>(&raw.x); b = *reinterpret_cast<const half2*>(&raw.y);
+                    }
+                    else
+                    {
+                        // rows too long for the cache: recompute the block (plain fp16 input only, checked on the host)
+                        const uint2 raw = __ldcg(reinterpret_cast<const uint2*>(reinterpret_cast<const half*>(o.A) + (size_t) r * o.k + c.kb * 128 + lane * 4));
+                        a = *reinterpret_cast<const half2*>(&raw.x); b = *reinterpret_cast<const half2*>(&raw.y);
                         if (o.suh)
                         {
-                            had128_warp(v0, v1, v2, v3, lane);
-                            a = __floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE);
-                            b = __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE);
-                            v0 = __low2float(a); v1 = __high2float(a); v2 = __low2float(b); v3 = __high2float(b);
+                            const uint2 scb = *reinterpret_cast<const uint2*>(o.suh + c.kb * 128 + lane * 4);
+                            a = __hmul2(a, *reinterpret_cast<const half2*>(&scb.x));
+                            b = __hmul2(b, *reinterpret_cast<const half2*>(&scb.y));
                         }
-                        uint32_t hi_w[4], lo_w[4];
-                        int qs = 0;
-                        i8_digits(v0, inv_scale[r], qs, hi_w[0], lo_w[0]);
-                        i8_digits(v1, inv_scale[r], qs, hi_w[1], lo_w[1]);
-                        i8_digits(v2, inv_scale[r], qs, hi_w[2], lo_w[2]);
-                        i8_digits(v3, inv_scale[r], qs, hi_w[3], lo_w[3]);
-                        // K order of the wgmma fragments (gemm_tc_i8_body.cuh): k = 4 lane + e -> K-chunk 16 (lane / 16) + 4 (lane % 4) + e,
-                        // byte 4 ((lane / 4) % 4)
-                        uint8_t* drow = dst + ((16 * (lane >> 4) + 4 * (lane & 3)) * 8 + 2 * r) * 16 + 4 * ((lane >> 2) & 3);
-                        #pragma unroll
-                        for (int e = 0; e < 4; ++e)
-                        {
-                            *reinterpret_cast<uint32_t*>(drow + e * 128) = hi_w[e];
-                            *reinterpret_cast<uint32_t*>(drow + e * 128 + 16) = lo_w[e];
-                        }
-                        qsum[r] = qs;
                     }
-                }
-                #pragma unroll
-                for (int d = 16; d > 0; d >>= 1)
-                {
-                    #pragma unroll
-                    for (int r = 0; r < CH_MR; ++r) qsum[r] += __shfl_xor_sync(0xffffffffu, qsum[r], d);
-                }
-                if (lane < o.m)
-                {
-                    int mine = 0;
-                    #pragma unroll
-                    for (int r = 0; r < CH_MR; ++r) if (lane == r) mine = qsum[r];
-                    *reinterpret_cast<int*>(dst + CH_B_BYTES + 4 * lane) = mine;
-                }
-                fence_proxy_async_smem();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(cx.X_FULL(s));
+                    if (o.suh)
+                    {
+                        float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
+                        had128_warp(v0, v1, v2, v3, lane);
+                        a = __floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE);
+                        b = __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE);
+                    }
+                    v[0] = __low2float(a); v[1] = __high2float(a); v[2] = __low2float(b); v[3] = __high2float(b);
+                });
                 CH_STAMP(c.seq == cx.trace_seq && lane == 0, 58);
             }
             if (++turn == CH_XF_WARPS) turn = 0;
@@ -562,18 +468,17 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
             c.next();
         }
     }
-    else if (warp >= CH_DEC_WARP0 && warp < CH_EPI_WARP0)
+    else if (warp >= TC_DEC_WARP0 && warp < TC_EPI_WARP0)
     {
         // =========================== decode groups: four warpgroups ===========================
         // warpgroup (g, nh): units seq = g (mod 2), output columns 64 nh .. 64 nh + 63; both groups hand over (possibly zero)
         // accumulators at every accumulation-chunk boundary, the epilogue adds the two
-        const int wq = warp & 3, wgi = (warp - CH_DEC_WARP0) >> 2;
+        const int wq = warp & 3, wgi = (warp - TC_DEC_WARP0) >> 2;
         const int g = wgi & 1, nh = wgi >> 1, tl = 4 * nh + wq;
-        const int chunk = lane >> 2, cq = lane & 3;
         Cursor c; c.init(ops, stages, p.n_stages, cta, G);
         int s = 0, ph = 0, dbuf = 0, dphase = 0;
         uint32_t acc[CH_MR] = {0u, 0u, 0u, 0u};
-        int tsum = 0;
+        int tsum = 0, t_hi = 0;                                          // t_hi: rows 4..7, none at MR = 4
         while (c.valid)
         {
             int sb, se; c.sub_bounds(sb, se);
@@ -583,30 +488,12 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                 const bool trace = c.seq == cx.trace_seq;
                 const int m = ops[c.op].m;
                 if constexpr (KSEL != 0) group_unit<KSEL>(cx, tl, lane, s, ph, m, acc, tsum, trace);
-                else
-                {
-                    switch (ops[c.op].K)
-                    {
-                        case 1: group_unit<1>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
-                        case 2: group_unit<2>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
-                        case 3: group_unit<3>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
-                        case 4: group_unit<4>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
-                        case 5: group_unit<5>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
-                        case 6: group_unit<6>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
-                        case 7: group_unit<7>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
-                        default: group_unit<8>(cx, tl, lane, s, ph, m, acc, tsum, trace); break;
-                    }
-                }
+                else EXL3B_DISPATCH_K(ops[c.op].K, group_unit<KK>(cx, tl, lane, s, ph, m, acc, tsum, trace));
             }
             if (last)
             {
                 mbar_wait(cx.D_EMPTY(dbuf), dphase ^ 1);               // the epilogue has drained this buffer
-                int32_t* dst = s_d + (size_t) ((dbuf * 2 + g) * 128 + 16 * tl + chunk) * (2 * CH_MR);
-                *reinterpret_cast<int2*>(dst + 2 * cq) = make_int2((int) acc[0], (int) acc[1]);
-                *reinterpret_cast<int2*>(dst + 8 * (2 * CH_MR) + 2 * cq) = make_int2((int) acc[2], (int) acc[3]);
-                if (tl == 0 && lane < 4) s_dt[(dbuf * 2 + g) * 8 + cq] = tsum;
-                acc[0] = acc[1] = acc[2] = acc[3] = 0u;
-                tsum = 0;
+                i8_hand_off<CH_MR>(s_d, s_dt, dbuf, g, nh, wq, lane, acc, tsum, t_hi);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(cx.D_FULL(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
@@ -615,19 +502,15 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
             c.next();
         }
     }
-    else if (warp >= CH_EPI_WARP0)
+    else if (warp >= TC_EPI_WARP0)
     {
         // =========================== epilogue ===========================
         pdl_wait();
         const int q = warp & 3;
-        const int et = threadIdx.x - CH_EPI_WARP0 * 32;
+        const int et = threadIdx.x - TC_EPI_WARP0 * 32;
         const int col = et;                                             // column of the strip this thread finishes
         float* tile = reinterpret_cast<float*>(smem + cx.L.off_tile);
         auto epi_bar = [] { asm volatile("bar.sync 1, 128;" ::: "memory"); };
-        const int part_stride = CH_MR * 128;
-        const float k_inv = __half2float(__ushort_as_half((unsigned short) 0x1eee));
-        const float k_bias = __half2float(__ushort_as_half((unsigned short) 0xc931));
-        const float c1 = 1534.0f * k_inv + k_bias;
         int dbuf = 0, dphase = 0, cur_op = -1;
         struct { void* C; const half* svh; long long unit_off; int m, n, KB, c_fp32; float out_scale; } o{};
         Cursor c; c.init(ops, stages, p.n_stages, cta, G);
@@ -642,25 +525,15 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
             }
             const int run_begin = c.run_begin, run_end = c.run_end;
             const long long U = stages[stage].U;
-            float* const parts = p.parts + (size_t) (stage & 1) * DevCtx::I8_PART_CTAS * part_stride;
+            // consecutive stages alternate between two exchange buffers
+            float* const parts = p.parts + (size_t) (stage & 1) * DevCtx::I8_PART_CTAS * (CH_MR * 128);
             float facc[CH_MR];
             #pragma unroll
             for (int r = 0; r < CH_MR; ++r) facc[r] = 0.f;
-            for (int sb = run_begin; sb < run_end; sb += CH_SUB_UNITS)
+            for (int sb = run_begin; sb < run_end; sb += I8_SUB_UNITS)
             {
                 mbar_wait<32>(cx.D_FULL(dbuf), dphase);
-                const int32_t* d0 = s_d + (size_t) ((dbuf * 2 + 0) * 128 + col) * (2 * CH_MR);
-                const int32_t* d1 = s_d + (size_t) ((dbuf * 2 + 1) * 128 + col) * (2 * CH_MR);
-                #pragma unroll
-                for (int r = 0; r < CH_MR; ++r)
-                {
-                    if (r < o.m)
-                    {
-                        const int T = s_dt[(dbuf * 2 + 0) * 8 + r] + s_dt[(dbuf * 2 + 1) * 8 + r];
-                        const long long sp = i8_centred_sum(d0[2 * r] + d1[2 * r], d0[2 * r + 1] + d1[2 * r + 1], T);
-                        facc[r] += i8_assemble(sp, T, s_scale[(op % CH_SCALE_SLOTS) * CH_MR + r], k_inv, c1);
-                    }
-                }
+                i8_drain<CH_MR>(s_d, s_dt, dbuf, col, o.m, [&](int r) { return s_scale[(op % CH_SCALE_SLOTS) * CH_MR + r]; }, facc);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(cx.D_EMPTY(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
@@ -670,71 +543,14 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
             const long long gs = o.unit_off + (long long) strip * o.KB;
             const int c_a = cta_of_unit((int) U, c.Gs, (int) gs), c_b = cta_of_unit((int) U, c.Gs, (int) (gs + o.KB - 1));
             const bool full = c_a == c_b;
-            bool emit = full;
             if (full)
             {
                 #pragma unroll
                 for (int r = 0; r < CH_MR; ++r) if (r < o.m) tile[r * 128 + col] = facc[r];
             }
-            else if (cta != c_a)
-            {
-                #pragma unroll
-                for (int r = 0; r < CH_MR; ++r)
-                    if (r < o.m)
-                    {
-                        uint32_t bits = __float_as_uint(facc[r]);
-                        if (bits == CH_SENTINEL) bits = 0x7fc00000u;
-                        st_relaxed_gpu_u32(reinterpret_cast<uint32_t*>(parts + (size_t) cta * part_stride + r * 128 + col), bits);
-                    }
-            }
-            else
-            {
-                #pragma unroll
-                for (int r = 0; r < CH_MR; ++r)
-                {
-                    if (r < o.m)
-                    {
-                        float a = facc[r];
-                        int cc0 = c_a + 1;
-                        while (cc0 <= c_b)
-                        {
-                            uint32_t v[8];
-                            bool ok;
-                            uint32_t polls = 0; unsigned long long t0 = 0;
-                            do
-                            {
-                                ok = true;
-                                #pragma unroll
-                                for (int j = 0; j < 8; ++j)
-                                {
-                                    const int cc = cc0 + j;
-                                    v[j] = 0u;
-                                    if (cc <= c_b)
-                                    {
-                                        v[j] = ld_relaxed_gpu_u32(reinterpret_cast<const uint32_t*>(parts + (size_t) cc * part_stride + r * 128 + col));
-                                        ok = ok && v[j] != CH_SENTINEL;
-                                    }
-                                }
-                                if (!ok) ch_watchdog(polls, t0, "split-K exchange", stage, strip);
-                            } while (!ok);
-                            #pragma unroll
-                            for (int j = 0; j < 8; ++j)
-                            {
-                                const int cc = cc0 + j;
-                                if (cc <= c_b)
-                                {
-                                    a += __uint_as_float(v[j]);
-                                    st_relaxed_gpu_u32(reinterpret_cast<uint32_t*>(parts + (size_t) cc * part_stride + r * 128 + col), CH_SENTINEL);
-                                }
-                            }
-                            cc0 += 8;
-                        }
-                        tile[r * 128 + col] = a;
-                    }
-                }
-                emit = true;
-            }
-            if (emit)
+            else if (cta != c_a) i8_splitk_publish<CH_MR>(parts, cta, facc, o.m, col);
+            else i8_splitk_reduce<CH_MR>(parts, 0, c_a, c_b, facc, o.m, col, tile);
+            if (full || cta == c_a)
             {
                 epi_bar();
                 for (int r = q; r < o.m; r += 4)
@@ -788,7 +604,7 @@ const char* chain_op_unsupported(int m, int k, int n, int K, int cb, int in_mode
     if (K < 1 || K > 8) return "K out of range";
     if (k < 128 || n < 128 || k % 128 || n % 128) return "k and n must be multiples of 128";
     if (in_mode < 0 || in_mode > 2) return "in_mode must be 0 (fp16 rows), 1 (silu(gate) * up, fp32) or 2 (same, fp16)";
-    if (in_mode != 0 && (size_t) m * k * 2 > CH_CACHE_MAX) return "gated input needs m * k <= 32768";
+    if (in_mode != 0 && (size_t) m * k * 2 > I8_CACHE_MAX_BYTES) return "gated input needs m * k <= 32768";
     return nullptr;
 }
 
@@ -822,9 +638,9 @@ static int chain_build(const exl3b_chain_op* in, int n_ops, int num_sms, Chain& 
         o.KB = a.k / 128; o.strips = a.n / 128; o.stage = (int) ch.stages.size() - 1;
         o.unit_off = st.U; o.out_scale = 1.0f;
         const size_t cb_ = ((size_t) a.m * a.k * 2 + 127) / 128 * 128;
-        o.cached = cb_ <= (size_t) CH_CACHE_MAX;
+        o.cached = cb_ <= (size_t) I8_CACHE_MAX_BYTES;
         if (o.cached && cb_ > cache) cache = cb_;
-        o.suh_cached = a.suh != nullptr && (size_t) a.k * 2 <= (size_t) CH_CACHE_MAX && ((uintptr_t) a.suh & 15) == 0;
+        o.suh_cached = a.suh != nullptr && (size_t) a.k * 2 <= (size_t) I8_CACHE_MAX_BYTES && ((uintptr_t) a.suh & 15) == 0;
         if (o.suh_cached && (size_t) a.k * 2 > suhb) suhb = (size_t) a.k * 2;
         if (o.cached && o.in_mode == 0 && ((uintptr_t) a.A & 15) != 0) o.cached = 0;      // bulk copy needs 16-byte alignment
         if (a.K < Kmin) Kmin = a.K;
@@ -834,8 +650,8 @@ static int chain_build(const exl3b_chain_op* in, int n_ops, int num_sms, Chain& 
     EXL3B_CHECK(ch.stages.size() <= 255, EXL3B_ERR_UNSUPPORTED, "exl3_chain: more than 255 stages");
     for (const ChainStage& st : ch.stages) if (st.U > Umax) Umax = st.U;
     const int w_bytes = 2048 * Kmax;
-    int S = (220 * 1024 - 128 - CH_MR * 128 * 4 - 2048 - CH_D_BYTES - (int) cache - (int) suhb) / (w_bytes + CH_B_STAGE);
-    if (S > CH_MAX_STAGES) S = CH_MAX_STAGES;
+    int S = (220 * 1024 - 128 - CH_MR * 128 * 4 - 2048 - i8_d_bytes(CH_MR) - (int) cache - (int) suhb) / (w_bytes + i8_b_stage(CH_MR));
+    if (S > TC_MAX_STAGES) S = TC_MAX_STAGES;
     EXL3B_CHECK(S >= 2, EXL3B_ERR_UNSUPPORTED, "exl3_chain: shared-memory budget exceeded");
     const ChainSmem L = chain_smem(S, w_bytes, (int) cache, (int) suhb);
     EXL3B_CHECK(L.total <= 220 * 1024, EXL3B_ERR_UNSUPPORTED, "exl3_chain: shared-memory budget exceeded");
@@ -850,40 +666,12 @@ static int chain_build(const exl3b_chain_op* in, int n_ops, int num_sms, Chain& 
     return 0;
 }
 
-template <int KSEL>
-static cudaError_t chain_launch_k(cudaStream_t stream, int grid, int smem_bytes, const ChainParams& p)
-{
-    static bool attr_set[32] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 31])
-    {
-        cudaError_t e = cudaFuncSetAttribute(chain_i8_kernel<KSEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set[dev & 31] = true;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(CH_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, chain_i8_kernel<KSEL>, p);
-}
-
 static cudaError_t chain_launch(cudaStream_t stream, int grid, int smem_bytes, const ChainParams& p, int ksel)
 {
-    switch (ksel)
-    {
-        case 1: return chain_launch_k<1>(stream, grid, smem_bytes, p);
-        case 2: return chain_launch_k<2>(stream, grid, smem_bytes, p);
-        case 3: return chain_launch_k<3>(stream, grid, smem_bytes, p);
-        case 4: return chain_launch_k<4>(stream, grid, smem_bytes, p);
-        case 5: return chain_launch_k<5>(stream, grid, smem_bytes, p);
-        case 6: return chain_launch_k<6>(stream, grid, smem_bytes, p);
-        case 7: return chain_launch_k<7>(stream, grid, smem_bytes, p);
-        case 8: return chain_launch_k<8>(stream, grid, smem_bytes, p);
-        default: return chain_launch_k<0>(stream, grid, smem_bytes, p);
-    }
+    cudaError_t err = cudaSuccess;
+    if (ksel == 0) err = launch_pdl<chain_i8_kernel<0>>(stream, dim3(grid), TC_THREADS, smem_bytes, p);
+    else EXL3B_DISPATCH_K(ksel, err = launch_pdl<chain_i8_kernel<KK>>(stream, dim3(grid), TC_THREADS, smem_bytes, p));
+    return err;
 }
 
 int chain_plan(const exl3b_chain_op* in, int n_ops, int num_sms, struct exl3b_chain_plan* out)

@@ -211,6 +211,42 @@ int launch_pack_trellis(cudaStream_t stream, uint16_t* packed, const uint16_t* u
         case 20: FN<5, 2>(__VA_ARGS__); break; case 21: FN<6, 2>(__VA_ARGS__); break;              \
         case 22: FN<7, 2>(__VA_ARGS__); break; case 23: FN<8, 2>(__VA_ARGS__); break;              \
     } } while (0)
+// K-only dispatch: runs the statement(s) with the compile-time constant KK = K (1..8)
+#define EXL3B_DISPATCH_K(K, ...)                                                                   \
+    do { switch (K) {                                                                              \
+        case 1: { constexpr int KK = 1; __VA_ARGS__; } break; case 2: { constexpr int KK = 2; __VA_ARGS__; } break; \
+        case 3: { constexpr int KK = 3; __VA_ARGS__; } break; case 4: { constexpr int KK = 4; __VA_ARGS__; } break; \
+        case 5: { constexpr int KK = 5; __VA_ARGS__; } break; case 6: { constexpr int KK = 6; __VA_ARGS__; } break; \
+        case 7: { constexpr int KK = 7; __VA_ARGS__; } break; case 8: { constexpr int KK = 8; __VA_ARGS__; } break; \
+    } } while (0)
+
+// ---- kernel launch helpers ------------------------------------------------------------------------------------
+// Raise KERNEL's dynamic shared-memory limit to `bytes`, once per device (the attribute belongs to the kernel on each device).
+template <auto KERNEL>
+cudaError_t set_max_smem_once(int bytes)
+{
+    static bool done[32] = {};
+    int dev = 0; cudaGetDevice(&dev);
+    if (done[dev & 31]) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) done[dev & 31] = true;
+    return e;
+}
+// Launch a kernel of up to 220 KiB dynamic shared memory with programmatic stream serialization (PDL): it may start while
+// the previous kernel of the stream finishes, so it must pdl_wait() before it reads that kernel's results.
+template <auto KERNEL, typename... Args>
+cudaError_t launch_pdl(cudaStream_t stream, dim3 grid, int threads, int smem_bytes, const Args&... args)
+{
+    const cudaError_t e = set_max_smem_once<KERNEL>(220 * 1024);
+    if (e != cudaSuccess) return e;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, KERNEL, args...);
+}
 
 // ---- device helpers -----------------------------------------------------------------------------------------
 #ifdef __CUDACC__

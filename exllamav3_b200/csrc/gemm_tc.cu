@@ -372,11 +372,6 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 
 int get_weight_tmap(const void* B, int k, int n, int K, CUtensorMap* out)
 {
-#ifdef EXL3B_TC_DEBUG
-    const bool flat = (g_tc_knob & 16) != 0;     // experiment: contiguous 8-row boxes (wrong data, same bytes)
-#else
-    constexpr bool flat = false;
-#endif
     static PFN_encodeTiled encode = nullptr;
     static std::mutex mu;
     struct Key { const void* p; int k, n, K; bool operator==(const Key& o) const { return p == o.p && k == o.k && n == o.n && K == o.K; } };
@@ -391,14 +386,13 @@ int get_weight_tmap(const void* B, int k, int n, int K, CUtensorMap* out)
         EXL3B_CHECK(fn && qres == cudaDriverEntryPointSuccess, EXL3B_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
         encode = (PFN_encodeTiled) fn;
     }
-    Key key{B, flat ? -k : k, n, K};
+    Key key{B, k, n, K};
     auto it = cache.find(key);
     if (it == cache.end())
     {
         CUtensorMap tm;
-        cuuint64_t row_bytes = (cuuint64_t) (n / 16) * 32 * K;
-        cuuint64_t rows = (cuuint64_t) (k / 16);
-        if (flat) { rows = rows * (n / 128); row_bytes = 256 * K; }
+        const cuuint64_t row_bytes = (cuuint64_t) (n / 16) * 32 * K;
+        const cuuint64_t rows = (cuuint64_t) (k / 16);
         cuuint64_t gdim[2] = { row_bytes / 8, rows };
         cuuint64_t gstride[1] = { row_bytes };
         cuuint32_t box[2] = { (cuuint32_t) (32 * K), 8 };
@@ -415,42 +409,19 @@ int get_weight_tmap(const void* B, int k, int n, int K, CUtensorMap* out)
 }
 
 template <int K, int cb>
-static cudaError_t tc_launch(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap)
-{
-    static bool attr_set[32] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 31])
-    {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<K, cb>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set[dev & 31] = true;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(XT_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, gemm_tc_kernel<K, cb>, p, tmap);
-}
-
-template <int K, int cb>
 static void tc_launch_v(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap,
                         cudaError_t* err)
 {
-    *err = tc_launch<K, cb>(stream, grid, smem_bytes, p, tmap);
+    *err = launch_pdl<gemm_tc_kernel<K, cb>>(stream, dim3(grid), XT_THREADS, smem_bytes, p, tmap);
 }
 
 unsigned long long* g_tc_dbg = nullptr;
-int g_tc_knob = 0;
 // bring-up hooks: live only in the EXL3B_TC_DEBUG build (libexl3b200_dbg.so); the production library ignores them, so no
 // exported call can change what its kernels compute
 #ifdef EXL3B_TC_DEBUG
 void tc_set_debug_buffer(unsigned long long* d) { g_tc_dbg = d; }
-void tc_set_knob(int k) { g_tc_knob = k; }
 #else
 void tc_set_debug_buffer(unsigned long long*) { }
-void tc_set_knob(int) { }
 #endif
 
 bool gemm_tc_supported(const GemmArgs& a)
@@ -550,7 +521,6 @@ int launch_gemm_tc(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
         p.b_load_bytes = pl.b_load_bytes;
         p.stages = pl.stages;
         p.dbg = g_tc_dbg;
-        p.knob_ = g_tc_knob;
         p.A_raw = fused_x ? a.A + (size_t) m0 * a.k : nullptr;
         p.suh = a.suh;
         p.b_bytes = pl.b_bytes;

@@ -13,30 +13,11 @@ gemm_tc_i8_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
 
 // ---- host side -------------------------------------------------------------------------------------------------------
 
-template <int K, int MR>
-static cudaError_t i8_launch_mr(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap)
-{
-    static bool attr_set[32] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 31])
-    {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tc_i8_kernel<K, MR>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set[dev & 31] = true;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, gemm_tc_i8_kernel<K, MR>, p, tmap);
-}
-
 template <int K>
 static cudaError_t i8_launch(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap)
 {
-    return p.m <= 4 ? i8_launch_mr<K, 4>(stream, grid, smem_bytes, p, tmap) : i8_launch_mr<K, 8>(stream, grid, smem_bytes, p, tmap);
+    return p.m <= 4 ? launch_pdl<gemm_tc_i8_kernel<K, 4>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap)
+                    : launch_pdl<gemm_tc_i8_kernel<K, 8>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap);
 }
 
 // rows 5..8 need the whole transformed activation cached in shared memory (the per-unit digit warps cannot afford eight Hadamards)
@@ -47,8 +28,8 @@ bool gemm_tc_i8_supported(const GemmArgs& a)
     return a.cb == 2 && i8_rows_ok(a.m, a.k) && a.k >= 128 && a.n >= 128 && a.k % 128 == 0 && a.n % 128 == 0;
 }
 
-// launch geometry (also behind exl3b_gemm_plan): rows variant, ring depth, activation cache, grid
-int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* pl)
+// rows variant, ring depth, activation cache and shared memory of a launch (single- and multi-matrix alike)
+static int plan_i8_smem(int m, int k, int K, TcPlan* pl)
 {
     const int MR = m <= 4 ? 4 : 8;
     const int stage_bytes = 2048 * K + i8_b_stage(MR);
@@ -60,6 +41,14 @@ int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPla
     if (stages < 2) stages = 2;
     const TcSmemLayout L = i8_smem_layout(K, MR, stages, cache_bytes);
     EXL3B_CHECK(L.total <= 220 * 1024, EXL3B_ERR_UNSUPPORTED, "exl3_gemm (i8): shared-memory budget exceeded");
+    pl->rows = MR; pl->stages = stages; pl->b_bytes = i8_b_stage(MR); pl->b_load_bytes = cache_bytes; pl->smem_total = L.total;
+    return 0;
+}
+
+// launch geometry (also behind exl3b_gemm_plan): rows variant, ring depth, activation cache, grid
+int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* pl)
+{
+    { int r = plan_i8_smem(m, k, K, pl); if (r) return r; }
     const long long U = (long long) (k / 128) * (n / 128);
     int grid = num_sms;
     if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
@@ -67,7 +56,6 @@ int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPla
     EXL3B_CHECK(n / 128 <= DevCtx::COUNTERS_PER_SLOT, EXL3B_ERR_UNSUPPORTED, "exl3_gemm: too many column strips");
     EXL3B_CHECK(grid <= DevCtx::I8_PART_CTAS, EXL3B_ERR_UNSUPPORTED, "exl3_gemm (i8): grid exceeds the split-K exchange buffer");
     EXL3B_CHECK(partition_fits(U, grid), EXL3B_ERR_UNSUPPORTED, "exl3_gemm (i8): too many units for the 32-bit stream-K partition");
-    pl->rows = MR; pl->stages = stages; pl->b_bytes = i8_b_stage(MR); pl->b_load_bytes = cache_bytes; pl->smem_total = L.total;
     pl->grid = grid; pl->units = U; pl->a_stages = 0; pl->d_bufs = 2; pl->tmem_cols = 0;
     return 0;
 }
@@ -82,22 +70,12 @@ int launch_gemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
     TcParams p{};
     p.B = a.B; p.C = a.C; p.svh = a.svh; p.m = a.m; p.k = a.k; p.n = a.n; p.NT = I8_NT; p.c_fp32 = a.c_fp32;
     p.out_scale = a.out_scale; p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot);
-    p.A_raw = a.A; p.suh = a.suh; p.dbg = g_tc_dbg; p.knob_ = g_tc_knob;
+    p.A_raw = a.A; p.suh = a.suh; p.dbg = g_tc_dbg;
     p.parts = ctx->i8_parts_slot(slot);
     p.stages = pl.stages; p.b_bytes = pl.b_bytes; p.b_load_bytes = pl.b_load_bytes;
     const int grid = pl.grid, smem_total = pl.smem_total;
     cudaError_t err = cudaSuccess;
-    switch (a.K)
-    {
-        case 1: err = i8_launch<1>(stream, grid, smem_total, p, tmap); break;
-        case 2: err = i8_launch<2>(stream, grid, smem_total, p, tmap); break;
-        case 3: err = i8_launch<3>(stream, grid, smem_total, p, tmap); break;
-        case 4: err = i8_launch<4>(stream, grid, smem_total, p, tmap); break;
-        case 5: err = i8_launch<5>(stream, grid, smem_total, p, tmap); break;
-        case 6: err = i8_launch<6>(stream, grid, smem_total, p, tmap); break;
-        case 7: err = i8_launch<7>(stream, grid, smem_total, p, tmap); break;
-        case 8: err = i8_launch<8>(stream, grid, smem_total, p, tmap); break;
-    }
+    EXL3B_DISPATCH_K(a.K, err = i8_launch<KK>(stream, grid, smem_total, p, tmap));
     count_launch();
     EXL3B_CUDA(err);
     EXL3B_CUDA(cudaPeekAtLastError());
@@ -163,24 +141,16 @@ int launch_mgemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a)
     TcParams p{};
     p.C = a.C; p.m = a.m; p.k = a.k; p.n = a.n; p.NT = I8_NT; p.c_fp32 = a.c_fp32;
     p.out_scale = 1.f; p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot);
-    p.A_raw = a.A; p.dbg = g_tc_dbg; p.knob_ = g_tc_knob;
+    p.A_raw = a.A; p.dbg = g_tc_dbg;
     p.num_mats = mats;                           // > 0 selects the table-driven path in the kernel
     p.B_ptrs = a.B_ptrs; p.suh_ptrs = a.suh_ptrs; p.svh_ptrs = a.svh_ptrs;
     p.a_mat_stride = a.bszm_in == 1 ? 0 : (long long) a.m * a.k;
     p.c_mat_stride = (long long) a.m * a.n * (a.c_fp32 ? 4 : 2);
     p.tmap_slots = ctx->tmap_slot(slot);
     p.parts = ctx->i8_parts_slot(slot);
-    const int MR = a.m <= 4 ? 4 : 8;
-    const int stage_bytes = 2048 * a.K + i8_b_stage(MR);
-    int cache_bytes = a.m * a.k * 2;
-    cache_bytes = (cache_bytes + 127) / 128 * 128;
-    if (cache_bytes > I8_CACHE_MAX_BYTES) cache_bytes = 0;
-    int stages = (200 * 1024 - i8_d_bytes(MR) - cache_bytes) / stage_bytes;
-    if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
-    if (stages < 2) stages = 2;
-    p.stages = stages; p.b_bytes = i8_b_stage(MR); p.b_load_bytes = cache_bytes;
-    const TcSmemLayout L = i8_smem_layout(a.K, MR, stages, cache_bytes);
-    EXL3B_CHECK(L.total <= 220 * 1024, EXL3B_ERR_UNSUPPORTED, "exl3_mgemm (i8): shared-memory budget exceeded");
+    TcPlan pl;
+    { int r = plan_i8_smem(a.m, a.k, a.K, &pl); if (r) return r; }
+    p.stages = pl.stages; p.b_bytes = pl.b_bytes; p.b_load_bytes = pl.b_load_bytes;
     const long long U = (long long) (a.k / 128) * (a.n / 128);
     int gpm = ctx->num_sms / mats;
     if (gpm > U) gpm = (int) U;
@@ -196,17 +166,7 @@ int launch_mgemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a)
         for (int j = 0; j < mats; ++j) p.rag_n[j] = a.size_n_host[j];
     }
     cudaError_t err = cudaSuccess;
-    switch (a.K)
-    {
-        case 1: err = i8_launch<1>(stream, grid, L.total, p, tmap); break;
-        case 2: err = i8_launch<2>(stream, grid, L.total, p, tmap); break;
-        case 3: err = i8_launch<3>(stream, grid, L.total, p, tmap); break;
-        case 4: err = i8_launch<4>(stream, grid, L.total, p, tmap); break;
-        case 5: err = i8_launch<5>(stream, grid, L.total, p, tmap); break;
-        case 6: err = i8_launch<6>(stream, grid, L.total, p, tmap); break;
-        case 7: err = i8_launch<7>(stream, grid, L.total, p, tmap); break;
-        case 8: err = i8_launch<8>(stream, grid, L.total, p, tmap); break;
-    }
+    EXL3B_DISPATCH_K(a.K, err = i8_launch<KK>(stream, grid, pl.smem_total, p, tmap));
     count_launch();
     EXL3B_CUDA(err);
     EXL3B_CUDA(cudaPeekAtLastError());

@@ -207,26 +207,6 @@ const char* gemm_tc_i8_ar_unsupported(int m, int k, int n, int K, int cb, int wo
     return nullptr;
 }
 
-template <int K>
-static cudaError_t i8_ar_launch(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap, const ArArgs& ar)
-{
-    static bool attr_set[32] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 31])
-    {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tc_i8_ar_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set[dev & 31] = true;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, gemm_tc_i8_ar_kernel<K>, p, tmap, ar);
-}
-
 // Same launch geometry as launch_gemm_tc_i8 (plan_gemm_tc_i8, gemm_tc_i8.cu); every rank must issue the same sequence of
 // row-parallel calls (the requirement any collective has).
 int launch_gemm_tc_i8_ar(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
@@ -241,7 +221,7 @@ int launch_gemm_tc_i8_ar(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
     TcParams p{};
     p.B = a.B; p.C = a.C; p.svh = a.svh; p.m = a.m; p.k = a.k; p.n = a.n; p.NT = I8_NT; p.c_fp32 = a.c_fp32;
     p.out_scale = a.out_scale; p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot);
-    p.A_raw = a.A; p.suh = a.suh; p.dbg = g_tc_dbg; p.knob_ = g_tc_knob;
+    p.A_raw = a.A; p.suh = a.suh; p.dbg = g_tc_dbg;
     p.parts = ctx->i8_parts_slot(slot);
     TcPlan pl;
     { int r = plan_gemm_tc_i8(a.m, a.k, a.n, a.K, ctx->num_sms, a.max_ctas, &pl); if (r) return r; }      // m <= 4: the MR = 4 variant
@@ -251,17 +231,7 @@ int launch_gemm_tc_i8_ar(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
     for (int j = 0; j < g->world; ++j) ar.recv[j] = g->recv[j];
     ar.state = g->state; ar.slot_elems = g->slot_elems; ar.rank = g->rank; ar.world = g->world;
     cudaError_t err = cudaSuccess;
-    switch (a.K)
-    {
-        case 1: err = i8_ar_launch<1>(stream, grid, pl.smem_total, p, tmap, ar); break;
-        case 2: err = i8_ar_launch<2>(stream, grid, pl.smem_total, p, tmap, ar); break;
-        case 3: err = i8_ar_launch<3>(stream, grid, pl.smem_total, p, tmap, ar); break;
-        case 4: err = i8_ar_launch<4>(stream, grid, pl.smem_total, p, tmap, ar); break;
-        case 5: err = i8_ar_launch<5>(stream, grid, pl.smem_total, p, tmap, ar); break;
-        case 6: err = i8_ar_launch<6>(stream, grid, pl.smem_total, p, tmap, ar); break;
-        case 7: err = i8_ar_launch<7>(stream, grid, pl.smem_total, p, tmap, ar); break;
-        case 8: err = i8_ar_launch<8>(stream, grid, pl.smem_total, p, tmap, ar); break;
-    }
+    EXL3B_DISPATCH_K(a.K, err = launch_pdl<gemm_tc_i8_ar_kernel<KK>>(stream, dim3(grid), TC_THREADS, pl.smem_total, p, tmap, ar));
     count_launch();
     EXL3B_CUDA(err);
     EXL3B_CUDA(cudaPeekAtLastError());

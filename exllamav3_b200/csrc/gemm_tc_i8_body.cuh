@@ -31,32 +31,9 @@
 //     matrix; the pointer tables stay in device memory, each CTA patches the weight tensor map's address on the device
 //   * instantiated for MR = 4 and MR = 8 activation rows (digit tile with one / two row groups); api.cu auto-selects m <= 4
 #pragma once
-#include "tc_common.cuh"
-#include "i8_math.cuh"
+#include "i8_pipeline.cuh"
 
 namespace exl3b {
-
-using namespace ptx;
-
-constexpr int I8_MAX_M = 8;                                    // rows per launch: kernel instantiated for MR = 4 and MR = 8 rows
-constexpr int I8_DEC_GROUPS = 2;
-constexpr int I8_NT = 16;                                      // N: rows 2r = hi digit, 2r+1 = lo digit of row r
-// digit tile of a unit: 32 K-chunks x (8 N-rows x 16 B) per row group; N-rows 2r / 2r+1 = hi / lo digit of activation row r, so
-// MR = 4 rows fill one row group (4096 B) and MR = 8 rows two (SBO = 4096 B); + 64 B of per-row digit sums behind the tile.
-// K order: the value of unit k-index 16 kt + 2 j + b (kt = 4 r + c) sits in K-chunk 2 (8 r + j) + b at byte 4 c -- the slot the
-// decode lane holding that weight feeds to wgmma (8 r + j).
-__host__ __device__ constexpr int i8_b_bytes(int MR) { return MR <= 4 ? 4096 : 8192; }
-__host__ __device__ constexpr int i8_b_stage(int MR) { return i8_b_bytes(MR) + 64; }
-constexpr int I8_SUB_UNITS = 96;                               // int32 accumulator safety: <= 12288 k per accumulation
-constexpr uint32_t I8_SENTINEL = 0xffffffffu;                  // "no partial sum here yet" in the split-K exchange buffer
-
-// optional shared-memory cache of the whole transformed activation (m x k fp16) and of the per-block digit sums, filled by
-// the CTA prologue: the per-unit transform then is an 8-byte LDS + quantise instead of a global load + Hadamard
-// (without it the two transform warps do a global load and a Hadamard per row and unit, on the per-unit critical path)
-constexpr int I8_CACHE_MAX_BYTES = 64 * 1024;
-
-// accumulator hand-off to the epilogue: [2 buffers][2 decode groups][128 columns][2 MR] int32, then [2][2][8] digit sums
-__host__ __device__ constexpr int i8_d_bytes(int MR) { return 2 * 2 * 128 * 2 * MR * 4 + 2 * 2 * 8 * 4; }
 
 __host__ __device__ inline TcSmemLayout i8_smem_layout(int K, int MR, int stages, int cache_bytes)
 {
@@ -153,11 +130,6 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     unsigned int* s_absmax = reinterpret_cast<unsigned int*>(misc + 4);           // [MR] float bits, >= 0
     [[maybe_unused]] volatile unsigned int* s_ar = reinterpret_cast<volatile unsigned int*>(misc + 28);   // AR: epoch of this launch
 
-#ifdef EXL3B_TC_DEBUG
-    const int KNOB = p.knob_;
-#else
-    constexpr int KNOB = 0;
-#endif
     auto stamp = [&](int slot)
     {
 #ifdef EXL3B_TC_DEBUG
@@ -349,58 +321,16 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         {
             I8_WAITCNT(wf_a, W_EMPTY(s), ph ^ 1);
             mbar_wait<64>(W_EMPTY(s), ph ^ 1);
-            uint8_t* dst = smem + L.off_b + s * L.b_bytes;
-            int qsum[MR];
-            #pragma unroll
-            for (int r = 0; r < MR; ++r)
+            i8_write_digit_tile<MR>(smem + L.off_b + s * L.b_bytes, inv_scale, p.m, lane, X_FULL(s), [&](int r, float (&v)[4])
             {
-                qsum[r] = 0;
-                if (r < p.m && !(KNOB & 8))
+                if (cached)
                 {
-                    float v[4];
-                    if (cached)
-                    {
-                        const uint2 raw = *reinterpret_cast<const uint2*>(xh_cache + (size_t) r * p.k + kb * 128 + lane * 4);
-                        const half2 a = *reinterpret_cast<const half2*>(&raw.x), b = *reinterpret_cast<const half2*>(&raw.y);
-                        v[0] = __low2float(a); v[1] = __high2float(a); v[2] = __low2float(b); v[3] = __high2float(b);
-                    }
-                    else xh_block(r, kb, v);
-                    uint32_t hi_w[4], lo_w[4];
-                    int qs = 0;
-                    #pragma unroll
-                    for (int e = 0; e < 4; ++e)
-                    {
-                        i8_digits(v[e], inv_scale[r], qs, hi_w[e], lo_w[e]);     // digits replicated over the 4 product bytes
-                    }
-                    // k = 4 lane + e: K-chunk 16 (lane / 16) + 4 (lane % 4) + e, byte 4 ((lane / 4) % 4); N-rows 2r (hi) and
-                    // 2r+1 (lo): row group r / 4, local rows 2 (r % 4), +1
-                    uint8_t* drow = dst + (r >> 2) * 4096 + ((16 * (lane >> 4) + 4 * (lane & 3)) * 8 + 2 * (r & 3)) * 16 + 4 * ((lane >> 2) & 3);
-                    #pragma unroll
-                    for (int e = 0; e < 4; ++e)
-                    {
-                        *reinterpret_cast<uint32_t*>(drow + e * 128) = hi_w[e];
-                        *reinterpret_cast<uint32_t*>(drow + e * 128 + 16) = lo_w[e];
-                    }
-                    qsum[r] = qs;
+                    const uint2 raw = *reinterpret_cast<const uint2*>(xh_cache + (size_t) r * p.k + kb * 128 + lane * 4);
+                    const half2 a = *reinterpret_cast<const half2*>(&raw.x), b = *reinterpret_cast<const half2*>(&raw.y);
+                    v[0] = __low2float(a); v[1] = __high2float(a); v[2] = __low2float(b); v[3] = __high2float(b);
                 }
-            }
-            // digit sums of all rows: the butterfly steps of different rows are independent, issued side by side
-            #pragma unroll
-            for (int o = 16; o > 0; o >>= 1)
-            {
-                #pragma unroll
-                for (int r = 0; r < MR; ++r) qsum[r] += __shfl_xor_sync(0xffffffffu, qsum[r], o);
-            }
-            if (lane < p.m)
-            {
-                int mine = 0;
-                #pragma unroll
-                for (int r = 0; r < MR; ++r) if (lane == r) mine = qsum[r];
-                *reinterpret_cast<int*>(dst + I8_B_BYTES + 4 * lane) = mine;
-            }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(X_FULL(s));
+                else xh_block(r, kb, v);
+            });
             kb += kstep; if (kb >= KB) kb -= KB;
             s += 2; if (s >= S) { s -= S; ph ^= 1; }
         }
@@ -416,7 +346,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         const int wq = warp & 3, wgi = (warp - TC_DEC_WARP0) >> 2;
         const int g = wgi & 1, nh = wgi >> 1;
         const int tl = 4 * nh + wq;                      // tile column of the strip owned by this warp
-        const int chunk = lane >> 2, c = lane & 3;
+        const int c = lane & 3;
         const uint64_t desc0 = smem_desc(smem_u32(smem + L.off_b), 128, 4096, 0);
         uint32_t acc[MR];
         #pragma unroll
@@ -441,28 +371,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                 const int* dsum = reinterpret_cast<const int*>(smem + L.off_b + s * L.b_bytes + I8_B_BYTES);
                 if (c < p.m) t_lo += dsum[c];
                 if (MR > 4 && c + 4 < p.m) t_hi += dsum[c + 4];
-                const uint64_t desc_s = desc0 + (uint64_t) ((s * L.b_bytes) >> 4);
-                #pragma unroll
-                for (int r = 0; r < 2; ++r)
-                {
-                    // the weight words of k-half r are loaded only now: one k-half's words and fragments are live at a time
-                    uint32_t w[K + 1], o0[16], o1[16];
-                    load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, w);
-                    decode16_i8<K, 0>(w, o0);
-                    decode16_i8<K, 1>(w, o1);
-                    #pragma unroll
-                    for (int i = 0; i < MR; ++i) reg_fence(acc[i]);
-                    wgmma_fence();
-                    #pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        wgmma_u8s8<MR>(acc, o0[2 * j], o1[2 * j], o0[2 * j + 1], o1[2 * j + 1], desc_s + (uint64_t) (16 * (8 * r + j)));
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    #pragma unroll
-                    for (int i = 0; i < 16; ++i) { reg_fence(o0[i]); reg_fence(o1[i]); }
-                    #pragma unroll
-                    for (int i = 0; i < MR; ++i) reg_fence(acc[i]);
-                }
+                i8_unit_mma<K, MR>(wst, desc0 + (uint64_t) ((s * L.b_bytes) >> 4), tl, lane, acc);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(W_EMPTY(s));
                 if (u == n_units - 1 && wq == 0 && lane == 0) stamp(10);
@@ -472,21 +381,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             {
                 // hand the sub-segment's accumulators to the epilogue
                 mbar_wait(D_EMPTY(dbuf), dphase ^ 1);
-                int32_t* dst = s_d + (size_t) ((dbuf * 2 + g) * 128 + 64 * nh + 16 * wq + chunk) * (2 * MR);
-                #pragma unroll
-                for (int i = 0; i < MR / 4; ++i)
-                {
-                    *reinterpret_cast<int2*>(dst + 8 * i + 2 * c) = make_int2((int) acc[4 * i], (int) acc[4 * i + 1]);
-                    *reinterpret_cast<int2*>(dst + 8 * (2 * MR) + 8 * i + 2 * c) = make_int2((int) acc[4 * i + 2], (int) acc[4 * i + 3]);
-                }
-                if (nh == 0 && wq == 0 && lane < 4)
-                {
-                    s_dt[(dbuf * 2 + g) * 8 + c] = t_lo;
-                    s_dt[(dbuf * 2 + g) * 8 + c + 4] = t_hi;
-                }
-                #pragma unroll
-                for (int i = 0; i < MR; ++i) acc[i] = 0u;
-                t_lo = 0; t_hi = 0;
+                i8_hand_off<MR>(s_d, s_dt, dbuf, g, nh, wq, lane, acc, t_lo, t_hi);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(D_FULL(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
@@ -504,13 +399,6 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         const int col = et;                              // column of the strip this thread finishes
         float* tile = reinterpret_cast<float*>(smem + L.off_tile);
         auto epi_bar = [] { asm volatile("bar.sync 1, 128;" ::: "memory"); };
-        const int part_stride = MR * 128;
-
-        // the prologue result is needed here too: wait for it through the first D_FULL (the MMA warp only gets
-        // operands after the transform warps passed the prologue barrier), then read the maxima
-        const float k_inv = __half2float(__ushort_as_half((unsigned short) 0x1eee));
-        const float k_bias = __half2float(__ushort_as_half((unsigned short) 0xc931));
-        const float c1 = 1534.0f * k_inv + k_bias;        // (1024 + 510) k_inv + k_bias: residue of the fp16-rounded bias
 
         // ---- AR: which exchange slot does this launch use?  ----------------------------------------------------------------
         // The slot must alternate between consecutive row-parallel launches of the rank (a peer may run one launch ahead, see
@@ -594,19 +482,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                             }
                         }
                         if (__all_sync(0xffffffffu, have == all)) break;
-                        if ((++polls & 255u) == 0)
-                        {
-                            unsigned long long t;
-                            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-                            if (t0 == 0) t0 = t;
-                            else if (t - t0 > 20000000000ull)
-                            {
-#if EXL3B_TC_DEBUG >= 2
-                                if (lane == 0) printf("exl3b: tensor-parallel exchange timeout (rank %d block %d strip %d have %x)\n", rank, blockIdx.x, strip, have);
-#endif
-                                __trap();
-                            }
-                        }
+                        poll_watchdog<255u, 20000000000ull>(polls, t0, "tensor-parallel exchange", strip, (int) have);
                     }
                     float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
                     #pragma unroll
@@ -655,21 +531,9 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                 const int sub = (seg - done) < I8_SUB_UNITS ? (seg - done) : I8_SUB_UNITS;
                 mbar_wait<32>(D_FULL(dbuf), dphase);
                 if (et == 0 && u + seg >= n_units) stamp(7);
-                const int32_t* d0 = s_d + (size_t) ((dbuf * 2 + 0) * 128 + col) * (2 * MR);
-                const int32_t* d1 = s_d + (size_t) ((dbuf * 2 + 1) * 128 + col) * (2 * MR);
-                #pragma unroll
-                for (int r = 0; r < MR; ++r)
-                {
-                    if (r < p.m)
-                    {
-                        const int T = s_dt[(dbuf * 2 + 0) * 8 + r] + s_dt[(dbuf * 2 + 1) * 8 + r];
-                        // sum_k q_k (bytesum_kn - 510), exact in 64-bit (the two groups' int32 partials add without loss)
-                        const long long sp = i8_centred_sum(d0[2 * r] + d1[2 * r], d0[2 * r + 1] + d1[2 * r + 1], T);
-                        const float mx = __uint_as_float(s_absmax[r]);
-                        const float scale = i8_over_qmax(mx);
-                        facc[r] += i8_assemble(sp, T, scale, k_inv, c1);
-                    }
-                }
+                // the prologue result is needed here too: the first D_FULL orders it (the MMA warps only get operands after the
+                // transform warps passed the prologue barrier)
+                i8_drain<MR>(s_d, s_dt, dbuf, col, p.m, [&](int r) { return i8_over_qmax(__uint_as_float(s_absmax[r])); }, facc);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(D_EMPTY(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
@@ -684,81 +548,14 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             }
             else if (cta != c_a)
             {
-                // Contributor: publish the partial sums and move on.  The data is its own flag: the exchange buffer holds the
-                // sentinel everywhere outside a launch, a 32-bit store is single-copy atomic, so no fence, counter or ticket.
-                #pragma unroll
-                for (int r = 0; r < MR; ++r)
-                    if (r < p.m)
-                    {
-                        uint32_t bits = __float_as_uint(facc[r]);
-                        if (bits == I8_SENTINEL) bits = 0x7fc00000u;                 // a NaN stays a NaN
-                        st_relaxed_gpu_u32(reinterpret_cast<uint32_t*>(parts + (size_t) (cta0 + cta) * part_stride + r * 128 + col), bits);
-                    }
+                // contributor: the exchange slots of this matrix's CTA group start at cta0
+                i8_splitk_publish<MR>(parts, cta0 + cta, facc, p.m, col);
                 if (et == 0 && u + seg >= n_units) stamp(11);
             }
             else
             {
-                // The CTA that owns the strip's FIRST k-segment works on it LAST (segments are processed in unit order), so it is the
-                // natural reducer: own sums from registers, then the others' in fixed CTA order (bit-reproducible).  One global
-                // round trip in the common case -- the old protocol needed three (fence + ticket, then the loads).
-                #pragma unroll
-                for (int r = 0; r < MR; ++r)
-                {
-                    if (r < p.m)
-                    {
-                        float a = 0.f;
-                        a += facc[r];
-                        int c = c_a + 1;
-                        while (c <= c_b)
-                        {
-                            uint32_t v[8];
-                            bool ok;
-                            uint32_t polls = 0;
-                            unsigned long long t0 = 0;
-                            do
-                            {
-                                ok = true;
-                                #pragma unroll
-                                for (int j = 0; j < 8; ++j)
-                                {
-                                    const int cc = c + j;
-                                    v[j] = 0u;
-                                    if (cc <= c_b)
-                                    {
-                                        v[j] = ld_relaxed_gpu_u32(reinterpret_cast<const uint32_t*>(parts + (size_t) (cta0 + cc) * part_stride + r * 128 + col));
-                                        ok = ok && v[j] != I8_SENTINEL;
-                                    }
-                                }
-                                if (!ok && (++polls & 255u) == 0)
-                                {
-                                    unsigned long long t;
-                                    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-                                    if (t0 == 0) t0 = t;
-                                    else if (t - t0 > 4000000000ull)
-                                    {
-#if EXL3B_TC_DEBUG >= 2
-                                        printf("exl3b: split-K exchange timeout (block %d strip %d)\n", blockIdx.x, strip);
-#endif
-                                        __trap();
-                                    }
-                                }
-                            } while (!ok);
-                            #pragma unroll
-                            for (int j = 0; j < 8; ++j)
-                            {
-                                const int cc = c + j;
-                                if (cc <= c_b)
-                                {
-                                    a += __uint_as_float(v[j]);
-                                    // re-arm the slot for the launch that uses this exchange buffer next (8 launches from now)
-                                    st_relaxed_gpu_u32(reinterpret_cast<uint32_t*>(parts + (size_t) (cta0 + cc) * part_stride + r * 128 + col), I8_SENTINEL);
-                                }
-                            }
-                            c += 8;
-                        }
-                        tile[r * 128 + col] = a;
-                    }
-                }
+                // reducer; its slots are re-armed for the launch that uses this exchange buffer next (8 launches from now)
+                i8_splitk_reduce<MR>(parts, cta0, c_a, c_b, facc, p.m, col, tile);
                 if (et == 0 && u + seg >= n_units) stamp(13);
                 emit_rows(strip);
             }

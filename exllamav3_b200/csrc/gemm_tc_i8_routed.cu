@@ -46,26 +46,6 @@ bool mgemm_tc_i8_routed_supported(const DevCtx* ctx, const MGemmArgs& a)
     return true;
 }
 
-template <int K>
-static cudaError_t i8_routed_launch(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap, const RouteArgs& route)
-{
-    static bool attr_set[32] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 31])
-    {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tc_i8_routed_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set[dev & 31] = true;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, gemm_tc_i8_routed_kernel<K>, p, tmap, route);
-}
-
 int launch_mgemm_tc_i8_routed(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a)
 {
     const int bszm = routed_slots(a);
@@ -83,7 +63,7 @@ int launch_mgemm_tc_i8_routed(cudaStream_t stream, DevCtx* ctx, const MGemmArgs&
     TcParams p{};
     p.C = a.C; p.m = a.m; p.k = a.k; p.n = a.n; p.NT = I8_NT; p.c_fp32 = a.c_fp32;
     p.out_scale = 1.f; p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot);
-    p.A_raw = a.A; p.dbg = g_tc_dbg; p.knob_ = g_tc_knob;
+    p.A_raw = a.A; p.dbg = g_tc_dbg;
     p.num_mats = bszm;
     p.B_ptrs = a.B_ptrs; p.suh_ptrs = a.suh_ptrs; p.svh_ptrs = a.svh_ptrs;
     p.a_mat_stride = a.bszm_in == 1 ? 0 : (long long) a.m * a.k;
@@ -96,17 +76,7 @@ int launch_mgemm_tc_i8_routed(cudaStream_t stream, DevCtx* ctx, const MGemmArgs&
     EXL3B_CHECK(grid <= DevCtx::I8_PART_CTAS && grid <= DevCtx::TMAP_SLOTS, EXL3B_ERR_UNSUPPORTED, "exl3_mgemm (routed i8): grid too large");
     RouteArgs route{tab, a.weights != nullptr ? 1 : 0};
     cudaError_t err = cudaSuccess;
-    switch (a.K)
-    {
-        case 1: err = i8_routed_launch<1>(stream, grid, pl.smem_total, p, tmap, route); break;
-        case 2: err = i8_routed_launch<2>(stream, grid, pl.smem_total, p, tmap, route); break;
-        case 3: err = i8_routed_launch<3>(stream, grid, pl.smem_total, p, tmap, route); break;
-        case 4: err = i8_routed_launch<4>(stream, grid, pl.smem_total, p, tmap, route); break;
-        case 5: err = i8_routed_launch<5>(stream, grid, pl.smem_total, p, tmap, route); break;
-        case 6: err = i8_routed_launch<6>(stream, grid, pl.smem_total, p, tmap, route); break;
-        case 7: err = i8_routed_launch<7>(stream, grid, pl.smem_total, p, tmap, route); break;
-        case 8: err = i8_routed_launch<8>(stream, grid, pl.smem_total, p, tmap, route); break;
-    }
+    EXL3B_DISPATCH_K(a.K, err = launch_pdl<gemm_tc_i8_routed_kernel<KK>>(stream, dim3(grid), TC_THREADS, pl.smem_total, p, tmap, route));
     count_launch();
     EXL3B_CUDA(err);
     if (a.weights)

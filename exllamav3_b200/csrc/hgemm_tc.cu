@@ -199,14 +199,9 @@ int launch_hgemm_tc(cudaStream_t stream, const half* a, const half* b, void* c, 
     HgParams p{};
     p.C = c; p.m = m; p.k = k; p.n = n; p.c_fp32 = c_fp32; p.c_stride = c_stride;
     p.tiles_m = (m + HG_BM - 1) / HG_BM; p.tiles_n = (n + HG_BN - 1) / HG_BN; p.k_iters = (k + HG_BK - 1) / HG_BK;
-    static bool attr_set[32] = {};
     int dev = 0; cudaGetDevice(&dev);
     const int smem_bytes = HG_STAGES * (HG_A_BYTES + HG_B_BYTES) + 256;
-    if (!attr_set[dev & 31])
-    {
-        EXL3B_CUDA(cudaFuncSetAttribute(hgemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-        attr_set[dev & 31] = true;
-    }
+    EXL3B_CUDA(set_max_smem_once<hgemm_tc_kernel>(smem_bytes));
     int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int grid = p.tiles_m * p.tiles_n; if (grid > sms) grid = sms;
     hgemm_tc_kernel<<<grid, HG_THREADS, smem_bytes, stream>>>(p, tmA, tmB);

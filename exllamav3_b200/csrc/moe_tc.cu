@@ -581,18 +581,7 @@ static cudaLaunchConfig_t moe_cfg(cudaStream_t stream, dim3 grid, int threads, i
 template <int K, int cb>
 static void moe_gemm_launch(cudaStream_t stream, int grid, const MoeGemmParams& p, cudaError_t* err)
 {
-    static bool attr_set[32] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    const int smem = moe_smem_layout(K, p.stages).total;
-    if (!attr_set[dev & 31])
-    {
-        *err = cudaFuncSetAttribute(moe_gemm_kernel<K, cb>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-        if (*err != cudaSuccess) return;
-        attr_set[dev & 31] = true;
-    }
-    cudaLaunchAttribute at[1];
-    cudaLaunchConfig_t cfg = moe_cfg(stream, dim3(grid), MOE_THREADS, smem, at);
-    *err = cudaLaunchKernelEx(&cfg, moe_gemm_kernel<K, cb>, p);
+    *err = launch_pdl<moe_gemm_kernel<K, cb>>(stream, dim3(grid), MOE_THREADS, moe_smem_layout(K, p.stages).total, p);
 }
 
 static int moe_gemm(cudaStream_t stream, const MoeWork& w, int chunk, long long grid_passes, const uint8_t* x,

@@ -59,14 +59,36 @@ __device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity)
                  : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0;
 }
-// Bounded wait: a protocol bug traps (reported as a CUDA error) instead of hanging the GPU.  The bound is wall-clock
-// (%globaltimer, checked every 1024 polls), not an iteration count: try_wait returns early whenever ANY barrier
-// activity wakes the warp, so iteration counts say nothing about elapsed time.
-// BACKOFF_NS > 0: exponential back-off (BACKOFF_NS, 2x, ... capped at 16x) between polls for roles whose waits can be
-// long: polling warps otherwise burn issue slots the decode warps need.
+// Watchdog of a bounded poll loop, called after every failed poll (polls and t0 start at 0): a protocol bug traps (reported
+// as a CUDA error) instead of hanging the GPU.  The bound is wall-clock (%globaltimer, read every MASK + 1 polls), not an
+// iteration count: an mbarrier try_wait returns early whenever ANY barrier activity wakes the warp, and a global-memory poll
+// takes as long as the memory system makes it, so iteration counts say nothing about elapsed time.
 // The timeout message is printed only in the bring-up build with messages (EXL3B_TC_DEBUG=2): printf is a function call, and any
 // call in a kernel that issues wgmma makes ptxas wait for every wgmma on its own (C7510), so the timeline build
 // (EXL3B_TC_DEBUG=1) leaves it out to time the production MMA schedule; the trap alone still ends the launch with an error.
+template <uint32_t MASK, unsigned long long LIMIT_NS = 4000000000ull>
+__device__ __forceinline__ void poll_watchdog(uint32_t& polls, unsigned long long& t0, const char* what, int a, int b)
+{
+    if ((++polls & MASK) == 0)
+    {
+        unsigned long long t;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+        if (t0 == 0) t0 = t;
+        else if (t - t0 > LIMIT_NS)
+        {
+#if EXL3B_TC_DEBUG >= 2
+            printf("exl3b: %s timeout (block %d thread %d: %d %d)\n", what, blockIdx.x, threadIdx.x, a, b);
+#else
+            (void) what; (void) a; (void) b;
+#endif
+            __trap();
+        }
+    }
+}
+
+// Bounded mbarrier wait (poll_watchdog, every 1024 polls).
+// BACKOFF_NS > 0: exponential back-off (BACKOFF_NS, 2x, ... capped at 16x) between polls for roles whose waits can be
+// long: polling warps otherwise burn issue slots the decode warps need.
 template <int BACKOFF_NS = 0>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
 {
@@ -77,19 +99,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
     while (!mbar_try_wait(bar, parity))
     {
         if constexpr (BACKOFF_NS > 0) { __nanosleep(ns); if (ns < 16u * BACKOFF_NS) ns <<= 1; }
-        if ((++polls & 1023u) == 0)
-        {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            if (t0 == 0) t0 = t;
-            else if (t - t0 > 4000000000ull)
-            {
-#if EXL3B_TC_DEBUG >= 2
-                printf("exl3b: mbarrier timeout (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
-#endif
-                __trap();
-            }
-        }
+        poll_watchdog<1023u>(polls, t0, "mbarrier", (int) bar, (int) parity);
     }
 }
 

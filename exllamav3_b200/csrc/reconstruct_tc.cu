@@ -205,14 +205,8 @@ template <int K, int cb>
 static void reconstruct_had_tc_launch(cudaStream_t stream, half* out, const uint16_t* packed, const half* suh, const half* svh,
                                       int k, int n_out, int packed_tiles_n, int tile_n_offset, int num_sms, cudaError_t* err)
 {
-    static bool attr_set[32] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 31])
-    {
-        *err = cudaFuncSetAttribute(reconstruct_had_tc_kernel<K, cb>, cudaFuncAttributeMaxDynamicSharedMemorySize, RT_SMEM);
-        if (*err != cudaSuccess) return;
-        attr_set[dev & 31] = true;
-    }
+    *err = set_max_smem_once<reconstruct_had_tc_kernel<K, cb>>(RT_SMEM);
+    if (*err != cudaSuccess) return;
     const int blocks_n = n_out / 128, n_blocks = blocks_n * (k / 128);
     int grid = 2 * num_sms; if (grid > n_blocks) grid = n_blocks;
     reconstruct_had_tc_kernel<K, cb><<<grid, RT_THREADS, RT_SMEM, stream>>>(out, (const uint32_t*) packed, suh, svh, n_out,

@@ -47,7 +47,6 @@ struct TcParams
     const uint64_t* c_ptrs;
     float* parts;                // i8 path: sentinel-managed split-K exchange buffer (one 4 x 128 fp32 slot per CTA)
     uint8_t* tmap_slots;         // one 128-byte tensor-map slot per CTA (global memory)
-    int knob_;                   // bring-up experiment switches (0 in production)
     unsigned long long* dbg;     // optional per-CTA timeline (16 x u64 per CTA), bring-up only
 };
 
@@ -129,6 +128,5 @@ __device__ __forceinline__ void store_tile_pair(uint8_t* p, uint2 o)
 
 int get_weight_tmap(const void* B, int k, int n, int K, CUtensorMap* out);
 extern unsigned long long* g_tc_dbg;
-extern int g_tc_knob;
 
 }  // namespace exl3b

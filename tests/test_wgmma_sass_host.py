@@ -112,3 +112,28 @@ def test_parser_flags_a_serialized_kernel():
     assert st["serialized"] == (2, 2, 1)
     assert st["half_serialized"] == (3, 1, 0)
     assert st["pipelined"] == (3, 0, 0)
+
+
+def test_timeline_build_keeps_wgmma_unserialized(tmp_path):
+    """The bring-up build with timeline stamps (EXL3B_TC_DEBUG=1) is the one the phase profiles time, so its int8 decode-GEMM
+    and chain kernels must issue the same unserialized wgmma as the production build: no CALL (a timeout printf) in them."""
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("exl3b_build", os.path.join(ROOT, "exllamav3_b200", "build.py"))
+    b = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(b)
+    flags = [f for f in b.NVCC_FLAGS if not f.startswith("-DEXL3B_TC_DEBUG")] + ["-DEXL3B_TC_DEBUG=1"]
+    exe = _cuobjdump()
+    seen, bad = 0, []
+    for s in ("gemm_tc_i8.cu", "chain_i8.cu"):
+        obj = str(tmp_path / s.replace(".cu", ".o"))
+        subprocess.run([b._nvcc(), "-c"] + flags + [os.path.join(b.CSRC, s), "-o", obj], check=True, capture_output=True)
+        sass = subprocess.run([exe, "-sass", obj], capture_output=True, text=True, check=True).stdout
+        for name, (n_mma, alone, calls) in kernel_stats(sass).items():
+            if n_mma == 0:
+                continue
+            seen += 1
+            if calls or alone:
+                bad.append(f"{s} {name}: {calls} CALL, {alone} of {n_mma} wgmma wait alone")
+    # 16 <K, MR> instantiations of the decode-GEMM, 9 of the chain
+    assert seen >= 25, f"only {seen} wgmma kernels found"
+    assert not bad, "\n".join(bad)

@@ -4,7 +4,7 @@ A/B of two builds of libexl3b200.so on the flagship workload: runs bench.py alte
 library (selected with EXL3B_LIBRARY), several times each in one process tree, and compares what both builds computed.
 
     python tools/ab_bench.py --baseline exllamav3_b200/libexl3b200_base.so [--candidate exllamav3_b200/libexl3b200.so]
-                             [--runs 3] [--steps 400] [--warmup 50] [--out DIR]
+                             [--mode ops|blocks|layer|token] [--runs 3] [--steps 400] [--warmup 50] [--out DIR]
 
 The baseline library is built from the old sources into its own directory and copied next to the candidate, e.g.
     git worktree add /tmp/base <commit>; (cd /tmp/base && EXL3B_LIB_SUFFIX=_base python -m exllamav3_b200.build)
@@ -23,10 +23,10 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def run_bench(lib, steps, warmup, dump_dir):
+def run_bench(lib, mode, steps, warmup, dump_dir):
     env = dict(os.environ, EXL3B_LIBRARY=os.path.abspath(lib))
     cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", str(steps), "--warmup", str(warmup),
-           "--dump-outputs", dump_dir]
+           "--mode", mode, "--dump-outputs", dump_dir]
     p = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=ROOT)
     lines = [ln for ln in p.stdout.splitlines() if ln.startswith("{")]
     if p.returncode != 0 or not lines:
@@ -58,6 +58,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--baseline", required=True)
     ap.add_argument("--candidate", default=os.path.join(ROOT, "exllamav3_b200", "libexl3b200.so"))
+    ap.add_argument("--mode", default="ops", help="bench.py --mode (blocks / layer / token run the chain kernel)")
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--steps", type=int, default=400)
     ap.add_argument("--warmup", type=int, default=50)
@@ -73,7 +74,7 @@ def main():
             order = list(builds) if i % 2 == 0 else list(reversed(builds))     # alternate which build goes first
             for name in order:
                 d = os.path.join(td, f"{name}_{i}")
-                runs[name].append(summary(run_bench(builds[name], args.steps, args.warmup, d)))
+                runs[name].append(summary(run_bench(builds[name], args.mode, args.steps, args.warmup, d)))
                 dumps.append(d)
                 print(f"run {i} {name}: {runs[name][-1]['value']:.1f} tok/s", file=sys.stderr, flush=True)
         n_out, diffs = 0, {}
@@ -83,7 +84,7 @@ def main():
                 diffs[os.path.basename(d)] = diff
     vals = {name: [r["value"] for r in rs] for name, rs in runs.items()}
     med = {name: statistics.median(v) for name, v in vals.items()}
-    line = {"runs": runs,
+    line = {"mode": args.mode, "runs": runs,
             "tok_s": {name: {"median": round(med[name], 1), "min": round(min(v), 1), "max": round(max(v), 1)} for name, v in vals.items()},
             "speedup_median": round(med["candidate"] / med["baseline"], 3),
             "outputs_compared": n_out, "outputs_bit_identical": not diffs, "differing_outputs": diffs}
