@@ -19,8 +19,10 @@
 //     reduction pass over the row by three warps (which also applies silu * mul for the gated-MLP input and caches
 //     x * suh in shared memory) replaces the 18-warp Hadamard prologue every CTA of the single-GEMM kernel runs.
 //     The 128-point Hadamard itself is done per unit by the digit warps from the cache, off the critical path.
-//     (|q| <= 32512 still holds; the scale is up to ~3x larger than the exact maximum, i.e. activations carry ~14.5
-//     instead of 16 bits: rel-RMS contribution 1e-4, tolerance tests in tests/test_chain.py.)
+//     (|q| <= 32512 still holds; on Gaussian rows the bound is ~3.5x the exact maximum (medians 3.3x .. 3.8x for
+//     k = 512 .. 14336, single rows 2.2x .. 4.7x), i.e. activations carry ~14 instead of 16 bits: rel-RMS
+//     contribution 1e-4.  The rule is modelled bit for bit by oracle.exl3_gemm_i8_model(rule="blocknorm"):
+//     tests/test_chain_host.py, tests/test_chain_exact.py.)
 //
 // Roles (768 threads): warp 0 TMA producer, warp 1 idle, warps 2-3 activation / digit warps, warps 4-19 decode + MMA (two
 // groups of two warpgroups), warps 20-23 epilogue; accumulators reach the epilogue through two shared-memory buffers.
@@ -624,6 +626,18 @@ static int chain_build(const exl3b_chain_op* in, int n_ops, int num_sms, Chain& 
         const char* why = chain_op_unsupported(a.m, a.k, a.n, a.K, a.cb, a.in_mode);
         EXL3B_CHECK(!why, EXL3B_ERR_UNSUPPORTED, "exl3_chain: op %d: %s", i, why ? why : "");
         EXL3B_CHECK(a.A && a.B && a.C && (a.in_mode == 0 || a.A2), EXL3B_ERR_ARG, "exl3_chain: op %d: null tensor", i);
+        // the kernel's vector accesses: fp32 gate / up by float4, fp16 rows / suh / svh by uint2, C by float4 (fp32) or uint2
+        // (fp16); k and n are multiples of 128, so an aligned base keeps every row aligned
+        {
+            const int a_align = a.in_mode == 1 ? 16 : 8, c_align = a.c_fp32 ? 16 : 8;
+            const char* bad = nullptr; int need = 0;
+            if ((uintptr_t) a.A % a_align) { bad = a.in_mode ? "gate (A)" : "A"; need = a_align; }
+            else if (a.in_mode != 0 && (uintptr_t) a.A2 % a_align) { bad = "up (A2)"; need = a_align; }
+            else if ((uintptr_t) a.suh % 8) { bad = "suh"; need = 8; }
+            else if ((uintptr_t) a.svh % 8) { bad = "svh"; need = 8; }
+            else if ((uintptr_t) a.C % c_align) { bad = "C"; need = c_align; }
+            EXL3B_CHECK(!bad, EXL3B_ERR_ARG, "exl3_chain: op %d: %s must be %d-byte aligned", i, bad ? bad : "", need);
+        }
         if (i == 0 || a.new_stage)
         {
             ChainStage st{};

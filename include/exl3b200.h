@@ -179,6 +179,10 @@ int exl3b_plan_fanout(int k, const int32_t* host_widths, int count, int num_sms,
  *                      activation_kernels.cuh:144-240, folded into down's input stage; result rounded to fp16 as there)
  *   B, suh, svh, C, m, k, n, K, cb, c_fp32   as exl3b_gemm (no A_had: the transform runs inside the kernel)
  * Eligibility per op: mul1 codebook, 1 <= m <= 4, k % 128 == n % 128 == 0; otherwise -EXL3B_ERR_UNSUPPORTED from create.
+ * Alignment per op (the kernel reads and writes these by 8- and 16-byte vectors): A 8 bytes (in_mode 0: 16 bytes lets the rows
+ * be staged in shared memory by one bulk copy, 8 runs uncached), gate / up 16 bytes (fp32) or 8 bytes (fp16), suh and svh 8 bytes
+ * (suh at 16 bytes is staged by a bulk copy), C 16 bytes (fp32) or 8 bytes (fp16); otherwise -EXL3B_ERR_ARG.  A contiguous view at
+ * an element offset, e.g. buf[1:].view(m, k), can miss these.
  * exl3b_chain_create copies the op table to the device (synchronous: call it outside stream capture, once per block, like the
  * reference constructs its BC_* modules once); exl3b_chain_run is one asynchronous launch, capturable in a CUDA graph;
  * returns EXL3B_TAG_TC_I8_CHAIN.  One chain runs at a time per device (stream order).

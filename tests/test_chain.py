@@ -7,7 +7,8 @@ CPU part: the kernel's own unit cursor replayed on the host (every unit of every
 and accumulation-chunk bounds, quad ownership), launch geometry, argument validation.
 GPU part: parity with the fp64 oracle (tolerances of README.md, Parity: max-abs <= 2e-3 max|y|, rel-RMS <= 1e-3) and with separate
 exl3_gemm calls, for single ops (every K, 1..4 rows, fp16 / fp32 outputs), same-input stages, dependent stages with the
-gated activation in between, at test sizes and at the Llama shapes.
+gated activation in between, at test sizes and at the Llama shapes; single ops also against the exact model of the kernel's
+arithmetic (oracle.exl3_gemm_i8_model, rule="blocknorm"; the rest of the chain's exact tests are in tests/test_chain_exact.py).
 """
 import ctypes
 import numpy as np
@@ -159,7 +160,7 @@ def _mk(k, n, K, m, dev, seed=0):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("K", [1, 2, 3, 4, 5, 6, 7, 8])
-@pytest.mark.parametrize("m", [1, 2, 4])
+@pytest.mark.parametrize("m", [1, 2, 3, 4])
 def test_chain_single_op_vs_oracle(cuda, K, m):
     from exllamav3_b200 import ext
     for (k, n, fp32) in ((512, 384, True), (1024, 256, False), (128, 128, True)):
@@ -172,6 +173,11 @@ def test_chain_single_op_vs_oracle(cuda, K, m):
         mx, rms = rel_err(y.cpu().numpy(), ref)
         tol = (2e-3, 1e-3) if fp32 else (4e-3, 2e-3)                     # fp16 C: + output rounding
         assert mx <= tol[0] and rms <= tol[1], (K, m, k, n, mx, rms)
+        # the exact model of the kernel's arithmetic (block-norm activation scale), per row
+        model = orc.exl3_gemm_i8_model(t["x"], t["tr"], t["suh"], t["svh"], K, rule="blocknorm")
+        for r in range(m):
+            mx, rms = rel_err(y[r:r + 1].cpu().numpy(), model[r:r + 1])
+            assert mx <= (2e-5 if fp32 else 1.5e-3) and rms <= (1e-5 if fp32 else 5e-4), (K, m, k, n, r, mx, rms)
         # replay: counters and exchange buffers re-armed
         y.zero_(); ch.run(); torch.cuda.synchronize()
         assert rel_err(y.cpu().numpy(), ref)[0] <= tol[0]
