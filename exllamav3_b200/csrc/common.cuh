@@ -172,9 +172,9 @@ int launch_hgemm(cudaStream_t stream, const half* a, const half* b, void* c, int
                  int64_t c_stride);
 
 // fused routed-expert MLP (moe_tc.cu, tag EXL3B_TAG_TC_MOE)
-constexpr int MOE_MAX_ROWS = 128;            // rows of one pass (the decode-GEMM's activation operand)
 constexpr int MOE_MAX_EXPERTS = 2048;
-// one pass: up to MOE_MAX_ROWS consecutive positions of one expert; row0 = its first row in chunk `chunk` of the work area
+// one pass: up to F16_MAX_ROWS (f16_pipeline.cuh) consecutive positions of one expert; row0 = its first row in chunk `chunk`
+// of the work area
 struct MoePass { int expert, pos0, rows, row0, chunk; };
 struct MoeArgs
 {
@@ -233,12 +233,16 @@ cudaError_t set_max_smem_once(int bytes)
     return e;
 }
 // Launch a kernel of up to 220 KiB dynamic shared memory with programmatic stream serialization (PDL): it may start while
-// the previous kernel of the stream finishes, so it must pdl_wait() before it reads that kernel's results.
+// the previous kernel of the stream finishes, so it must pdl_wait() before it reads that kernel's results.  Only a launch
+// beyond the default 48 KiB raises the kernel's limit: a kernel with large static shared memory could not take the raise.
 template <auto KERNEL, typename... Args>
 cudaError_t launch_pdl(cudaStream_t stream, dim3 grid, int threads, int smem_bytes, const Args&... args)
 {
-    const cudaError_t e = set_max_smem_once<KERNEL>(220 * 1024);
-    if (e != cudaSuccess) return e;
+    if (smem_bytes > 48 * 1024)
+    {
+        const cudaError_t e = set_max_smem_once<KERNEL>(220 * 1024);
+        if (e != cudaSuccess) return e;
+    }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
     cudaLaunchAttribute at[1];

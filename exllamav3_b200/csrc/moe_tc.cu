@@ -15,15 +15,13 @@
 //   7. reduce   output_state[t] += w_j * d_j over the token's positions of the chunk in ascending j.  Chunks cover ascending
 //               position ranges, so every token's sum runs in ascending j whatever the chunking: deterministic, no atomics
 //
-// The GEMM is the tag-200 decode-GEMM (gemm_tc.cu): decoded weights are the wgmma A fragments (m64n16k16, fp32 accumulation),
-// activations the N = 16..128 operand.  It differs in two ways.  An item covers the whole k range of one strip, so there is no
-// split-K exchange and the accumulators go straight to the output transform.  Weights and activations arrive by plain 1-D
-// bulk copies (eight 256K-byte trellis rows per 128 x 128 unit) from addresses read out of the device pointer tables: no tensor
-// map has to be encoded on the host or patched per CTA and fenced when a CTA moves to another expert.
-#include "common.cuh"
-#include "decode.cuh"
-#include "epilogue.cuh"
-#include "tc_common.cuh"
+// The GEMM is tag 200's unit (layout and helpers in f16_pipeline.cuh): decoded weights are the wgmma A fragments (m64n16k16,
+// fp32 accumulation), activations the N = 16..128 operand.  Its own parts are the producer and the epilogue.  An item covers the
+// whole k range of one strip, so there is no split-K exchange and the accumulators go straight to the output transform.
+// Weights and activations arrive by plain 1-D bulk copies (eight 256K-byte trellis rows per 128 x 128 unit) from addresses
+// read out of the device pointer tables: no tensor map has to be encoded on the host or patched per CTA and fenced when a
+// CTA moves to another expert.
+#include "f16_pipeline.cuh"
 #include <mutex>
 #include <vector>
 
@@ -31,16 +29,13 @@ namespace exl3b {
 
 using namespace ptx;
 
-constexpr int MOE_THREADS = 384;                 // warp 0 producer, warps 4-11 decode + MMA + epilogue (two warpgroups)
-constexpr int MOE_CONS_WARP0 = 4, MOE_CONS_WARPS = 8;
 constexpr int MOE_ROUTE_THREADS = 1024;
-constexpr int MOE_B_BYTES = MOE_MAX_ROWS * 256;  // activation stage: 128 rows x 128 k fp16
 
 __host__ __device__ inline int moe_padded(int rows) { return (rows + 15) & ~15; }
 
 // The work list of one call.  Experts in index order; an expert is processed when 0 < c_e <= T and its positions lie inside
 // [end of the previous processed expert, num_positions), so processed ranges are disjoint and ascending even for malformed
-// counts.  Each processed expert is cut into passes of <= MOE_MAX_ROWS consecutive positions; passes are packed in order into
+// counts.  Each processed expert is cut into passes of <= F16_MAX_ROWS consecutive positions; passes are packed in order into
 // chunks of at most chunk_rows padded rows.  The same function runs in the route kernel and behind exl3b_moe_plan.
 struct MoePlanArrays
 {
@@ -68,9 +63,9 @@ __host__ __device__ inline bool moe_plan(const long long* count, int E, int T, i
         if (moe_processed(c, s, lo, T, N))
         {
             a.p_start[np] = (int) s; a.p_rows[np] = (int) c; a.p_pass0[np] = P; ++np;
-            for (int r0 = 0; r0 < (int) c; r0 += MOE_MAX_ROWS)
+            for (int r0 = 0; r0 < (int) c; r0 += F16_MAX_ROWS)
             {
-                const int rows = (int) c - r0 < MOE_MAX_ROWS ? (int) c - r0 : MOE_MAX_ROWS;
+                const int rows = (int) c - r0 < F16_MAX_ROWS ? (int) c - r0 : F16_MAX_ROWS;
                 const int pad = moe_padded(rows);
                 if (R + pad > chunk_rows)
                 {
@@ -104,7 +99,7 @@ __host__ __device__ inline int moe_pos_code(int j, int np, const int* p_start, c
     const int i = lo - 1;
     if (i < 0 || j >= p_start[i] + p_rows[i]) return -1;
     const int r = j - p_start[i];
-    return (p_pass0[i] + r / MOE_MAX_ROWS) * 128 + r % MOE_MAX_ROWS;
+    return (p_pass0[i] + r / F16_MAX_ROWS) * 128 + r % F16_MAX_ROWS;
 }
 
 // ---- fixed per-device work area ------------------------------------------------------------------------------------------
@@ -112,7 +107,7 @@ __host__ __device__ inline int moe_pos_code(int j, int np, const int* p_start, c
 // work-list region bounds one call's positions and tokens; the row region holds one chunk's tiles and rows, so larger calls
 // run in more chunks instead of needing more memory.
 constexpr long long MOE_MAX_POSITIONS = 1 << 20;        // positions and tokens of one call
-constexpr int MOE_MAX_PASSES = MOE_MAX_EXPERTS + (int) (MOE_MAX_POSITIONS / MOE_MAX_ROWS);
+constexpr int MOE_MAX_PASSES = MOE_MAX_EXPERTS + (int) (MOE_MAX_POSITIONS / F16_MAX_ROWS);
 constexpr int MOE_MAX_CHUNKS = 4096;
 constexpr size_t MOE_ROW_BYTES = (size_t) 240 << 20;
 
@@ -131,7 +126,7 @@ static MoeBounds moe_bounds(long long N, long long E, long long T, int chunk_row
 {
     MoeBounds b;
     const long long np = N < E * T ? N : E * T;
-    b.passes = np < E + np / MOE_MAX_ROWS ? np : E + np / MOE_MAX_ROWS;
+    b.passes = np < E + np / F16_MAX_ROWS ? np : E + np / F16_MAX_ROWS;
     b.rows = np + 15 * b.passes;
     b.chunks = b.rows == 0 ? 0 : 1 + b.rows / (chunk_rows - 112);
     return b;
@@ -226,18 +221,8 @@ moe_route_kernel(MoeWork w, const int64_t* __restrict__ expert_count, const int6
 }
 
 // ---- 2. gather + input transform --------------------------------------------------------------------------------------------
-// One warp per (position, 128-k block): x[token] * suh -> Hadamard -> fp16 into the pass's tile (the tag-200 input transform,
-// gemm_tc.cu had_tiled_kernel).  Pass p's tiles start at row0 * k fp16; block kb of it is NT * 256 bytes.
-__device__ __forceinline__ uint2 moe_transform(uint2 raw, const half* suh, int lane)
-{
-    half2 a = *reinterpret_cast<half2*>(&raw.x), b = *reinterpret_cast<half2*>(&raw.y);
-    const uint2 scb = *reinterpret_cast<const uint2*>(suh);
-    a = __hmul2(a, *reinterpret_cast<const half2*>(&scb.x));
-    b = __hmul2(b, *reinterpret_cast<const half2*>(&scb.y));
-    float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
-    had128_warp(v0, v1, v2, v3, lane);
-    return pack_tile_pair(__floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE), __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE));
-}
+// One warp per (position, 128-k block): x[token] through the tag-200 input transform (xt_transform) into the pass's tile.
+// Pass p's tiles start at row0 * k fp16; block kb of it is NT * 256 bytes.
 
 __global__ void __launch_bounds__(128)
 moe_gather_kernel(MoeWork w, const half* __restrict__ x, const int64_t* __restrict__ token_sorted,
@@ -260,8 +245,8 @@ moe_gather_kernel(MoeWork w, const half* __restrict__ x, const int64_t* __restri
     if (t >= 0 && t < bsz) raw = *reinterpret_cast<const uint2*>(x + (size_t) t * k + kb * 128 + lane * 4);
     const size_t off = (size_t) ps.row0 * k * 2 + (size_t) kb * moe_padded(ps.rows) * 256 + xt_tile_offset(r, lane);
     const int c0 = kb * 128 + lane * 4;
-    if (gated) store_tile_pair(xg + off, moe_transform(raw, (const half*) suh_g[ps.expert] + c0, lane));
-    store_tile_pair(xu + off, moe_transform(raw, (const half*) suh_u[ps.expert] + c0, lane));
+    if (gated) store_tile_pair(xg + off, xt_transform(raw, (const half*) suh_g[ps.expert] + c0, lane));
+    store_tile_pair(xu + off, xt_transform(raw, (const half*) suh_u[ps.expert] + c0, lane));
 }
 
 // ---- 3, 4, 6. grouped decode-GEMM ---------------------------------------------------------------------------------------------
@@ -275,25 +260,12 @@ struct MoeGemmParams
     int k, n, stages;
 };
 
-__host__ __device__ inline TcSmemLayout moe_smem_layout(int K, int stages)
-{
-    TcSmemLayout L;
-    L.w_bytes = 2048 * K;
-    L.b_bytes = MOE_B_BYTES;
-    L.off_b = stages * L.w_bytes;
-    L.off_tile = L.off_b + stages * L.b_bytes;
-    L.off_bars = L.off_tile + MOE_MAX_ROWS * 128 * 4;
-    L.total = L.off_bars + 1024;
-    L.off_d = L.total;
-    return L;
-}
-
 template <int K, int cb>
-__global__ void __launch_bounds__(MOE_THREADS, 1)
+__global__ void __launch_bounds__(F16_THREADS, 1)
 moe_gemm_kernel(const MoeGemmParams p)
 {
     extern __shared__ __align__(1024) uint8_t smem[];
-    const TcSmemLayout L = moe_smem_layout(K, p.stages);
+    const TcSmemLayout L = f16_smem_layout(K, F16_MAX_ROWS * 256, p.stages, F16_MAX_ROWS);
     // values broadcast from lane 0 are warp-uniform to ptxas: without that, a loop bound or wgmma predicate loaded from memory
     // counts as divergent and ptxas serializes the wgmma (C7520)
     auto uni = [](int v) { return __shfl_sync(0xffffffffu, v, 0); };
@@ -306,7 +278,7 @@ moe_gemm_kernel(const MoeGemmParams p)
     pdl_launch_dependents();
     if (warp == 0)
     {
-        for (int s = lane; s < S; s += 32) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), MOE_CONS_WARPS); }
+        for (int s = lane; s < S; s += 32) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), F16_CONS_WARPS); }
         fence_barrier_init();
     }
     __syncthreads();
@@ -349,19 +321,19 @@ moe_gemm_kernel(const MoeGemmParams p)
             }
         }
     }
-    else if (warp >= MOE_CONS_WARP0)
+    else if (warp >= F16_CONS_WARP0)
     {
         // =========================== decode + MMA + epilogue (two warpgroups) ===========================
-        const int ct = threadIdx.x - MOE_CONS_WARP0 * 32;
+        const int ct = threadIdx.x - F16_CONS_WARP0 * 32;
         const int cw = ct >> 5;
         const int h = cw >> 2, wq = cw & 3;
         const int tl = 4 * h + wq;
         const int chunk = lane >> 2, c = lane & 3;
         float* tile = reinterpret_cast<float*>(smem + L.off_tile);
         auto cons_bar = [] { asm volatile("bar.sync 1, 256;" ::: "memory"); };
-        const uint64_t desc0 = smem_desc(smem_u32(smem + L.off_b), 128, 2048, 0);
+        const uint64_t desc0 = f16_tile_desc(smem + L.off_b);
 
-        float acc[MOE_MAX_ROWS / 16][8];
+        float acc[F16_MAX_ROWS / 16][8];
         int s = 0, sph = 0;
         for (int it = blockIdx.x; it < items; it += G)
         {
@@ -369,18 +341,13 @@ moe_gemm_kernel(const MoeGemmParams p)
             const MoePass ps = p.passes[pass0 + pi];
             const int expert = uni(ps.expert), rows = uni(ps.rows), row0 = uni(ps.row0);
             const int nchunks = moe_padded(rows) / 16;
-            #pragma unroll
-            for (int i = 0; i < MOE_MAX_ROWS / 16; ++i)
-                #pragma unroll
-                for (int e = 0; e < 8; ++e) acc[i][e] = 0.f;
+            f16_zero(acc);
 
             for (int kb = 0; kb < KB; ++kb)
             {
                 mbar_wait<32>(FULL(s), sph);
-                const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
                 uint32_t wr[2][K + 1];
-                #pragma unroll
-                for (int r = 0; r < 2; ++r) load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, wr[r]);
+                f16_load_unit<K>(reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes), tl, chunk, c, wr);
                 const uint64_t desc_s = desc0 + (uint64_t) ((s * L.b_bytes) >> 4);
                 #pragma unroll
                 for (int r = 0; r < 2; ++r)
@@ -389,15 +356,16 @@ moe_gemm_kernel(const MoeGemmParams p)
                     decode16<K, cb, 0>(wr[r], o0);
                     decode16<K, cb, 1>(wr[r], o1);
                     #pragma unroll
-                    for (int ii = 0; ii < MOE_MAX_ROWS / 16; ++ii)
+                    for (int ii = 0; ii < F16_MAX_ROWS / 16; ++ii)
                         #pragma unroll
                         for (int e = 0; e < 8; ++e) reg_fence(acc[ii][e]);
                     wgmma_fence();
                     #pragma unroll
                     for (int j = 0; j < 4; ++j)
                     {
+                        // instruction 4 r + j: K-chunks 2 (4 r + j), +1;  N-chunk ii: row groups 2 ii, 2 ii + 1
                         #pragma unroll
-                        for (int ii = 0; ii < MOE_MAX_ROWS / 16; ++ii)
+                        for (int ii = 0; ii < F16_MAX_ROWS / 16; ++ii)
                             if (ii < nchunks)
                                 wgmma_f16_n16(acc[ii], o0[2 * j], o1[2 * j], o0[2 * j + 1], o1[2 * j + 1],
                                               desc_s + (uint64_t) (16 * (4 * r + j) + 256 * ii));
@@ -407,7 +375,7 @@ moe_gemm_kernel(const MoeGemmParams p)
                     #pragma unroll
                     for (int e = 0; e < 8; ++e) { reg_fence(o0[e]); reg_fence(o1[e]); }
                     #pragma unroll
-                    for (int ii = 0; ii < MOE_MAX_ROWS / 16; ++ii)
+                    for (int ii = 0; ii < F16_MAX_ROWS / 16; ++ii)
                         #pragma unroll
                         for (int e = 0; e < 8; ++e) reg_fence(acc[ii][e]);
                 }
@@ -416,28 +384,12 @@ moe_gemm_kernel(const MoeGemmParams p)
                 if (++s == S) { s = 0; sph ^= 1; }
             }
 
-            // accumulators -> tile[row][column] -> output transform of the pass's rows (gemm_tc.cu's layout)
+            // accumulators -> tile -> output transform of the pass's rows
             cons_bar();                                              // the previous item's epilogue has read the tile
-            const int n0 = 16 * tl + chunk;
-            #pragma unroll
-            for (int ii = 0; ii < MOE_MAX_ROWS / 16; ++ii)
-            {
-                if (ii < nchunks)
-                {
-                    const int r0 = 16 * ii + 2 * c;
-                    tile[(r0 + 0) * 128 + n0] = acc[ii][0];
-                    tile[(r0 + 1) * 128 + n0] = acc[ii][1];
-                    tile[(r0 + 0) * 128 + n0 + 8] = acc[ii][2];
-                    tile[(r0 + 1) * 128 + n0 + 8] = acc[ii][3];
-                    tile[(r0 + 8) * 128 + n0] = acc[ii][4];
-                    tile[(r0 + 9) * 128 + n0] = acc[ii][5];
-                    tile[(r0 + 8) * 128 + n0 + 8] = acc[ii][6];
-                    tile[(r0 + 9) * 128 + n0 + 8] = acc[ii][7];
-                }
-            }
+            f16_store_tile(tile, acc, tl, chunk, c, nchunks);
             cons_bar();
             const half* svh = reinterpret_cast<const half*>(p.svh_ptrs[expert]) + strip * 128;
-            for (int j = cw; j < rows; j += MOE_CONS_WARPS)
+            for (int j = cw; j < rows; j += F16_CONS_WARPS)
                 output_row_128(tile + j * 128, (char*) p.C, (size_t) (row0 + j) * p.n + strip * 128, svh, 1.0f, p.c_fp32 != 0, lane);
         }
     }
@@ -486,7 +438,7 @@ moe_act_kernel(MoeWork w, const half* __restrict__ g, const half* __restrict__ u
     uint2 raw;
     raw.x = pack_half2(hv[0], hv[1]); raw.y = pack_half2(hv[2], hv[3]);
     const size_t off = (size_t) ps.row0 * k * 2 + (size_t) kb * moe_padded(ps.rows) * 256 + xt_tile_offset(r, lane);
-    store_tile_pair(xd + off, moe_transform(raw, (const half*) suh_d[ps.expert] + kb * 128 + lane * 4, lane));
+    store_tile_pair(xd + off, xt_transform(raw, (const half*) suh_d[ps.expert] + kb * 128 + lane * 4, lane));
 }
 
 // ---- 7. fixed-order weighted sum into output_state ------------------------------------------------------------------------
@@ -553,35 +505,17 @@ static int moe_limits(long long N, int E, int T, long long bsz, int hidden, int 
     const long long kb = (hidden > inter ? hidden : inter) / 128;
     EXL3B_CHECK(N * kb * 32 <= 0x7fffffffll, EXL3B_ERR_UNSUPPORTED, "exl3_moe: positions x width too large for one call");
     *chunk_rows = moe_chunk_rows(hidden, inter);
-    EXL3B_CHECK(*chunk_rows >= 2 * MOE_MAX_ROWS, EXL3B_ERR_UNSUPPORTED, "exl3_moe: hidden %d / intermediate %d too large for the work area",
+    EXL3B_CHECK(*chunk_rows >= 2 * F16_MAX_ROWS, EXL3B_ERR_UNSUPPORTED, "exl3_moe: hidden %d / intermediate %d too large for the work area",
                 hidden, inter);
     *b = moe_bounds(N, E, T, *chunk_rows);
     EXL3B_CHECK(b->passes <= MOE_MAX_PASSES && b->chunks <= MOE_MAX_CHUNKS, EXL3B_ERR_UNSUPPORTED, "exl3_moe: work list too long");
     return 0;
 }
 
-static int moe_stages(int K)
-{
-    const int budget = 200 * 1024 - MOE_MAX_ROWS * 128 * 4;
-    int st = budget / (2048 * K + MOE_B_BYTES);
-    if (st > TC_MAX_STAGES) st = TC_MAX_STAGES;
-    return st < 2 ? 2 : st;
-}
-
-static cudaLaunchConfig_t moe_cfg(cudaStream_t stream, dim3 grid, int threads, int smem, cudaLaunchAttribute* at)
-{
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cfg;
-}
-
 template <int K, int cb>
 static void moe_gemm_launch(cudaStream_t stream, int grid, const MoeGemmParams& p, cudaError_t* err)
 {
-    *err = launch_pdl<moe_gemm_kernel<K, cb>>(stream, dim3(grid), MOE_THREADS, moe_smem_layout(K, p.stages).total, p);
+    *err = launch_pdl<moe_gemm_kernel<K, cb>>(stream, dim3(grid), F16_THREADS, f16_smem_layout(K, F16_MAX_ROWS * 256, p.stages, F16_MAX_ROWS).total, p);
 }
 
 static int moe_gemm(cudaStream_t stream, const MoeWork& w, int chunk, long long grid_passes, const uint8_t* x,
@@ -590,7 +524,7 @@ static int moe_gemm(cudaStream_t stream, const MoeWork& w, int chunk, long long 
     MoeGemmParams p{};
     p.hdr = w.hdr; p.passes = w.passes; p.chunk_first = w.chunk_first; p.chunk = chunk;
     p.x = x; p.B_ptrs = B_ptrs; p.svh_ptrs = svh_ptrs; p.C = C; p.c_fp32 = c_fp32;
-    p.k = k; p.n = n; p.stages = moe_stages(K);
+    p.k = k; p.n = n; p.stages = f16_stages(K, F16_MAX_ROWS);
     const long long items = grid_passes * (n / 128);
     const int grid = items < num_sms ? (int) items : num_sms;
     cudaError_t err = cudaSuccess;
@@ -664,24 +598,17 @@ int launch_moe(cudaStream_t stream, DevCtx* ctx, const MoeArgs& a)
     // persistent grids: a chunk has at most chunk_rows / 16 passes; num_active (processed experts, if the caller knows it)
     // narrows that further
     long long grid_passes = b.passes < chunk_rows / 16 ? b.passes : chunk_rows / 16;
-    if (a.num_active > 0 && a.num_active + N / MOE_MAX_ROWS < grid_passes) grid_passes = a.num_active + N / MOE_MAX_ROWS;
+    if (a.num_active > 0 && a.num_active + N / F16_MAX_ROWS < grid_passes) grid_passes = a.num_active + N / F16_MAX_ROWS;
 
-    cudaLaunchAttribute at[1];
-    cudaError_t e;
-    {
-        cudaLaunchConfig_t cfg = moe_cfg(stream, dim3(1), MOE_ROUTE_THREADS, 0, at);
-        e = cudaLaunchKernelEx(&cfg, moe_route_kernel, w, a.expert_count, a.token_sorted, a.num_experts, a.max_tokens,
-                               a.num_positions, a.bsz, chunk_rows, (int) b.passes, (int) b.chunks);
-        count_launch(); EXL3B_CUDA(e);
-    }
+    cudaError_t e = launch_pdl<moe_route_kernel>(stream, dim3(1), MOE_ROUTE_THREADS, 0, w, a.expert_count, a.token_sorted,
+                                                 a.num_experts, a.max_tokens, a.num_positions, a.bsz, chunk_rows, (int) b.passes,
+                                                 (int) b.chunks);
+    count_launch(); EXL3B_CUDA(e);
     for (int c = 0; c < (int) b.chunks; ++c)
     {
-        {
-            cudaLaunchConfig_t cfg = moe_cfg(stream, dim3((unsigned) ((N * KBh + 3) / 4)), 128, 0, at);
-            e = cudaLaunchKernelEx(&cfg, moe_gather_kernel, w, a.hidden_state, a.token_sorted, a.gate_suh, a.up_suh, xg, xu,
-                                   a.num_positions, a.hidden, a.bsz, gated, c);
-            count_launch(); EXL3B_CUDA(e);
-        }
+        e = launch_pdl<moe_gather_kernel>(stream, dim3((unsigned) ((N * KBh + 3) / 4)), 128, 0, w, a.hidden_state, a.token_sorted,
+                                          a.gate_suh, a.up_suh, xg, xu, a.num_positions, a.hidden, a.bsz, gated, c);
+        count_launch(); EXL3B_CUDA(e);
         int r;
         if (gated)
         {
@@ -690,19 +617,14 @@ int launch_moe(cudaStream_t stream, DevCtx* ctx, const MoeArgs& a)
         }
         r = moe_gemm(stream, w, c, grid_passes, xu, a.up_trellis, a.up_svh, u, 0, a.hidden, a.inter, a.K_up, a.cb, ctx->num_sms);
         if (r) return r;
-        {
-            cudaLaunchConfig_t cfg = moe_cfg(stream, dim3((unsigned) ((N * KBi + 3) / 4)), 128, 0, at);
-            e = cudaLaunchKernelEx(&cfg, moe_act_kernel, w, (const half*) g, (const half*) u, a.down_suh, xd, a.num_positions,
-                                   a.inter, a.act, a.act_limit, c);
-            count_launch(); EXL3B_CUDA(e);
-        }
+        e = launch_pdl<moe_act_kernel>(stream, dim3((unsigned) ((N * KBi + 3) / 4)), 128, 0, w, (const half*) g, (const half*) u,
+                                       a.down_suh, xd, a.num_positions, a.inter, a.act, a.act_limit, c);
+        count_launch(); EXL3B_CUDA(e);
         r = moe_gemm(stream, w, c, grid_passes, xd, a.down_trellis, a.down_svh, d, 1, a.inter, a.hidden, a.K_down, a.cb, ctx->num_sms);
         if (r) return r;
-        {
-            cudaLaunchConfig_t cfg = moe_cfg(stream, dim3(a.bsz, (a.hidden + 511) / 512), 128, 0, at);
-            e = cudaLaunchKernelEx(&cfg, moe_reduce_kernel, w, a.output_state, a.weight_sorted, (const float*) d, a.hidden, c);
-            count_launch(); EXL3B_CUDA(e);
-        }
+        e = launch_pdl<moe_reduce_kernel>(stream, dim3(a.bsz, (a.hidden + 511) / 512), 128, 0, w, a.output_state, a.weight_sorted,
+                                          (const float*) d, a.hidden, c);
+        count_launch(); EXL3B_CUDA(e);
     }
     EXL3B_CUDA(cudaPeekAtLastError());
     return EXL3B_TAG_TC_MOE;

@@ -1,4 +1,4 @@
-// Shared declarations of the tensor-core kernels (exact fp16 path: gemm_tc.cu, int8 codebook path: gemm_tc_i8.cu).
+// Shared declarations of the tensor-core kernels (exact fp16 path: gemm_tc.cu, moe_tc.cu; int8 codebook path: gemm_tc_i8.cu).
 #pragma once
 #include "common.cuh"
 #include "decode.cuh"
@@ -30,7 +30,7 @@ struct TcParams
     int stages;                  // smem ring depth
     int b_bytes;                 // bytes reserved per activation stage
     int b_load_bytes;            // bytes of the activation tile copied per unit
-    const half* A_raw;           // fused input transform (m <= 8): raw activations (m, k) and suh; null -> xh_tiled is used
+    const half* A_raw;           // int8 kernels: raw activations (m, k), transformed in-kernel with suh
     const half* suh;
     // multi-matrix launch (exl3_mgemm, dense case): the grid is num_mats groups of g_per_mat CTAs, group j works on
     // matrix j exactly like a single-matrix launch with g_per_mat CTAs.  num_mats == 0: single matrix, fields unused.
@@ -123,6 +123,18 @@ __device__ __forceinline__ void store_tile_pair(uint8_t* p, uint2 o)
 {
     *reinterpret_cast<uint32_t*>(p) = o.x;
     *reinterpret_cast<uint32_t*>(p + 128) = o.y;
+}
+// The input transform of lane's four values k = 4 lane .. 4 lane + 3 of one row (raw fp16, one 128-k block per warp):
+// * suh (`suh` points at lane's four scales) -> 128-point Hadamard in fp32 -> * 1/sqrt(128) -> fp16, as a tile pair
+__device__ __forceinline__ uint2 xt_transform(uint2 raw, const half* suh, int lane)
+{
+    half2 a = *reinterpret_cast<half2*>(&raw.x), b = *reinterpret_cast<half2*>(&raw.y);
+    const uint2 scb = *reinterpret_cast<const uint2*>(suh);
+    a = __hmul2(a, *reinterpret_cast<const half2*>(&scb.x));
+    b = __hmul2(b, *reinterpret_cast<const half2*>(&scb.y));
+    float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
+    had128_warp(v0, v1, v2, v3, lane);
+    return pack_tile_pair(__floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE), __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE));
 }
 #endif
 

@@ -1,7 +1,7 @@
 """
 Decode-GEMM kernels at the geometry edges (H100): every template instantiation, every accumulator row group and pass count,
 forced persistent grids that produce every split-K pattern, the uncached int8 activations, the int32 accumulation chunks at
-their worst case, the fused input transform and CUDA-graph replay.  Which branch each shape reaches is asserted on the host
+their worst case and CUDA-graph replay.  Which branch each shape reaches is asserted on the host
 in tests/test_edges_host.py, which also holds the shared tables and input builders.  The oracle is given each decoded weight
 (exl3_gemm_f64's w, exl3_gemm_i8_model's bsum) so that it decodes once per matrix, not once per call.
 
@@ -12,9 +12,6 @@ Bars (README.md, Parity): vs oracle.exl3_gemm_f64 max-abs <= 2e-3 max|y| (+1 fp1
 exact model oracle.exl3_gemm_i8_model max-abs <= 2e-5 max|y|, rel-RMS <= 1e-5 (fp32 C), 1.5e-3 / 5e-4 (fp16 C).
 """
 import contextlib
-import os
-import subprocess
-import sys
 import numpy as np
 import pytest
 import torch
@@ -23,7 +20,6 @@ from test_edges_host import CACHE_PAIRS, FORCED_GRIDS, WORST_KQ, gemm_plan, wors
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TAG_SIMT, TAG_TC, TAG_I8, TAG_CHAIN = 100, 200, 210, 220
 SENTINEL = {torch.half: (torch.int16, 0x7E5A), torch.float: (torch.int32, 0x7FA5A5A5)}     # NaN payloads nobody writes
 
@@ -342,52 +338,7 @@ def test_int8_worst_case_int32_accumulation(cuda):
         check_f64(y, ref, True, (m, "chain"))
 
 
-# ---- 6. the fused input transform ----------------------------------------------------------------------------------------
-
-FUSED_KQ_CB = ((1, 0), (4, 2), (8, 1))
-FUSED_KB = (1, 2, 3, 5)
-FUSED_GRIDS = (0, 2)
-
-
-def fused_transform_outputs(dev):
-    """fp32 outputs of tag 200 for every fused-transform case, keyed by case; plus the shared-memory plan of one case."""
-    from exllamav3_b200 import ext
-    out = {}
-    with gemm_path(TAG_TC):
-        for (K, cb) in FUSED_KQ_CB:
-            for KB in FUSED_KB:
-                tr, suh, svh, x = orc.make_synthetic(128 * KB, 384, K, m=8, seed=800 + 10 * K + KB)
-                mt = Mat(dev, tr, suh, svh, K, cb)
-                for m in range(1, 9):
-                    for G in FUSED_GRIDS:
-                        out[f"{K}_{cb}_{KB}_{m}_{G}"] = run(ext, dev, x[:m], mt, True, force=G)[0]
-    out["plan_smem"] = np.array([gemm_plan(4, 512, 384, 4, 0).smem_bytes])
-    return out
-
-
-def test_fused_input_transform_is_bit_identical(cuda, tmp_path):
-    """
-    EXL3B_FUSED_X_ROWS (read once per process) moves the input transform of up to 8 rows into two warps of the kernel.  Both
-    transforms do the same arithmetic (__hmul2, had128_warp, R_SCALE, round to nearest) and feed wgmma the same valid rows, so the
-    child process's outputs must equal the tiled path's here bit for bit.
-    """
-    assert os.environ.get("EXL3B_FUSED_X_ROWS", "0") in ("", "0"), "this process must run the default tiled transform"
-    env = dict(os.environ, EXL3B_FUSED_X_ROWS="8")
-    code = ("import sys, numpy as np, torch; sys.path[:0] = [sys.argv[1], sys.argv[1] + '/tests']; import test_gpu_edges as t; "
-            "np.savez(sys.argv[2], **t.fused_transform_outputs(torch.device('cuda:0')))")
-    out_path = str(tmp_path / "fused.npz")
-    r = subprocess.run([sys.executable, "-c", code, ROOT, out_path], env=env, timeout=900, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    fused = np.load(out_path)
-    tiled = fused_transform_outputs(cuda)
-    # the child really planned the fused variant: its activation stage is one 2 KiB row group instead of NT * 256 bytes
-    assert fused["plan_smem"][0] != tiled["plan_smem"][0]
-    for key, y in tiled.items():
-        if key != "plan_smem":
-            assert np.array_equal(fused[key].view(np.uint64), y.view(np.uint64)), key
-
-
-# ---- 7. CUDA-graph replay ------------------------------------------------------------------------------------------------
+# ---- 6. CUDA-graph replay ------------------------------------------------------------------------------------------------
 
 def test_graph_replay_matches_eager(cuda):
     """

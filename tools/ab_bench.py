@@ -12,8 +12,8 @@ The baseline library is built from the old sources into its own directory and co
 (a build product like the candidate, so git ignores it).  Every run writes its outputs with --dump-outputs; the script requires
 them to be bit-identical across all runs of both builds (the int8 path accumulates integers, so a reordering of the MMAs changes
 no bit).  It prints one
-JSON line: per build the tok/s of every run, the per-launch qgemm times of gate, down and lm_head, and the reference's own
-kernels timed in the same bench runs.
+JSON line: per build the tok/s of every run, the per-launch qgemm times of gate, down and lm_head, of the batch-8 / 32 decode
+and of the other two codebooks, and the reference's own kernels timed in the same bench runs.
 """
 from __future__ import annotations
 import argparse, glob, json, os, statistics, subprocess, sys, tempfile
@@ -35,10 +35,14 @@ def run_bench(lib, mode, steps, warmup, dump_dir):
 
 
 def summary(res):
-    q = (res.get("qgemm") or {}).get("decode_hbm", {})
-    ref = ((res.get("qgemm") or {}).get("reference_cuda") or {}).get("shapes", {})
+    qg = res.get("qgemm") or {}
+    q = qg.get("decode_hbm", {})
+    ref = (qg.get("reference_cuda") or {}).get("shapes", {})
+    times = lambda d: {k: {"us": v["us_per_launch"], "GBps": v["GBps"]} for k, v in d.items()}
+    # decode_batch (m = 8 / 32) and decode_codebooks (3inst / mcg at m = 1) are where bench.py times the fp16 path (tag 200)
     return {"value": res["value"],
-            "decode_hbm": {k: {"us": v["us_per_launch"], "GBps": v["GBps"]} for k, v in q.items() if k in ("gate", "down", "lm_head")},
+            "decode_hbm": {k: v for k, v in times(q).items() if k in ("gate", "down", "lm_head")},
+            "decode_batch": times(qg.get("decode_batch", {})), "decode_codebooks": times(qg.get("decode_codebooks", {})),
             "reference_cuda": ref}
 
 
