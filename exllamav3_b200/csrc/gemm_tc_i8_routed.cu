@@ -10,8 +10,10 @@
 // It replaces the CUDA-core contraction that the default path (launch_mgemm, tag 100) runs between the same two bookkeeping
 // kernels; semantics are those of exl3_gemm.cu:341-381.
 //
-// Tests: tests/test_moe_routed.py (five routing modes vs the oracle and vs the CUDA-core twin,
-// Mixtral expert shapes); selected automatically for routed mul1 calls at <= 4 rows, the CUDA-core kernels take the rest.
+// Tests: tests/test_moe_routed.py (five routing modes vs the oracle and vs the CUDA-core twin, Mixtral expert shapes) and
+// tests/test_moe_routed_exact.py (every slot vs the exact int8 model and bit for bit vs tag 210, the reduce bit for bit at
+// num_tokens >= 1, shards, 1..128 slots, graph replay); selected automatically for routed mul1 calls at <= 4 rows, the
+// CUDA-core kernels take the rest.
 #include "gemm_tc_i8_body.cuh"
 
 namespace exl3b {
