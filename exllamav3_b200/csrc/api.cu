@@ -3,6 +3,7 @@
 #include "common.cuh"
 #include "epilogue.cuh"
 #include "tc_common.cuh"
+#include "act.cuh"
 #include <mutex>
 #include <unordered_map>
 #include <vector>
@@ -278,6 +279,46 @@ int exl3b_gemm(void* stream_, const void* A, const void* B, void* C, const void*
     if (path == EXL3B_TAG_TC_I8) return launch_gemm_tc_i8(stream, ctx, g);
     if (path == EXL3B_TAG_TC) return launch_gemm_tc(stream, ctx, g);
     return launch_gemm_simt(stream, ctx, g);
+}
+
+int exl3b_act_mul(void* stream, const void* g, const void* u, void* a, int64_t numel, int in_fp32, int act, float act_limit)
+{
+    EXL3B_CHECK(act >= ACT_SILU && act <= ACT_RELU2, EXL3B_ERR_ARG, "act_mul: act must be 0 (SiLU), 1 (GELU) or 2 (ReLU^2), got %d", act);
+    EXL3B_CHECK(numel >= 0, EXL3B_ERR_SHAPE, "act_mul: negative size");
+    if (numel == 0) return 0;
+    EXL3B_CHECK(g && u && a, EXL3B_ERR_ARG, "act_mul: null tensor");
+    DevCtx* ctx; int r = get_ctx(&ctx); if (r) return r;
+    return launch_act_mul((cudaStream_t) stream, g, u, (half*) a, (long long) numel, in_fp32 != 0, act, act_limit);
+}
+
+// exl3b_gemm on the rows fp16(act(G) * U): the path exl3b_gemm takes for (m, k, n, K, cb), restricted to the two kernels with a
+// gated input stage (tag 210 at m <= 4, tag 200 at m <= 8); any other choice is refused, never replaced
+int exl3b_gemm_gated(void* stream, const void* G, const void* U, const void* B, void* C, const void* suh, const void* svh,
+                     int m, int k, int n, int K, int cb, int c_fp32, int gu_fp32, int act, float act_limit, int force_num_sms)
+{
+    int r = check_kcb(K, cb); if (r) return r;
+    EXL3B_CHECK(act >= ACT_SILU && act <= ACT_RELU2, EXL3B_ERR_ARG, "exl3_gemm_gated: act must be 0 (SiLU), 1 (GELU) or 2 (ReLU^2), got %d", act);
+    EXL3B_CHECK(m >= 0 && k >= 0 && n >= 0, EXL3B_ERR_SHAPE, "exl3_gemm_gated: negative size");
+    EXL3B_CHECK(k % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm_gated: k (%d) must be divisible by 128", k);
+    EXL3B_CHECK(n % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm_gated: n (%d) must be divisible by 128", n);
+    if (m == 0 || n == 0) return EXL3B_TAG_NOP;
+    EXL3B_CHECK(m <= 8, EXL3B_ERR_UNSUPPORTED, "exl3_gemm_gated: gated input is implemented for 1..8 rows, got %d", m);
+    EXL3B_CHECK(G && U && B && C, EXL3B_ERR_ARG, "exl3_gemm_gated: null tensor");
+    const uintptr_t align = gu_fp32 ? 16 : 8;
+    EXL3B_CHECK((uintptr_t) G % align == 0 && (uintptr_t) U % align == 0, EXL3B_ERR_ARG,
+                "exl3_gemm_gated: G and U must be %d-byte aligned", (int) align);
+    GemmArgs g{};
+    g.A = nullptr; g.suh = (const half*) suh; g.A_had = nullptr; g.B = (const uint32_t*) B; g.C = C; g.svh = (const half*) svh;
+    g.m = m; g.k = k; g.n = n; g.K = K; g.cb = cb; g.c_fp32 = c_fp32 != 0; g.out_scale = 1.0f;
+    g.max_ctas = force_num_sms > 0 ? force_num_sms : 0;
+    const int path = select_gemm_path(g);
+    if (path < 0) return path;
+    EXL3B_CHECK(path == EXL3B_TAG_TC || (path == EXL3B_TAG_TC_I8 && m <= 4), EXL3B_ERR_UNSUPPORTED,
+                "exl3_gemm_gated: the call selects path %d at m = %d; gated input exists on paths 210 (m <= 4) and 200", path, m);
+    GateIn gate{G, U, gu_fp32 != 0, act, act_limit};
+    DevCtx* ctx; r = get_ctx(&ctx); if (r) return r;
+    if (path == EXL3B_TAG_TC_I8) return launch_gemm_tc_i8((cudaStream_t) stream, ctx, g, &gate);
+    return launch_gemm_tc((cudaStream_t) stream, ctx, g, &gate);
 }
 
 int exl3b_gemm_allreduce(void* stream_, const void* A, const void* B, void* C, const void* suh, void* A_had, const void* svh,

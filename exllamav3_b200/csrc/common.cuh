@@ -120,9 +120,11 @@ int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPla
 int plan_gemm_tc(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* pl);     // m <= 256: one pass
 
 int launch_gemm_simt(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a);
-int launch_gemm_tc(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a);
+// gate != null (exl3b_gemm_gated, act.cuh): the kernel's rows are fp16(act(G) * U) instead of a.A
+struct GateIn;
+int launch_gemm_tc(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a, const GateIn* gate = nullptr);
 bool gemm_tc_supported(const GemmArgs& a);
-int launch_gemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a);
+int launch_gemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a, const GateIn* gate = nullptr);
 struct MGemmArgs;
 bool mgemm_tc_i8_supported(const DevCtx* ctx, const MGemmArgs& a);
 int launch_mgemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a);
@@ -167,6 +169,9 @@ int launch_mgemm_reduce(cudaStream_t stream, DevCtx* ctx, const MSlotTable* tab,
 // routed / weighted exl3_mgemm (MoE decode) on the wgmma int8 path (gemm_tc_i8_routed.cu): opt-in, tag EXL3B_TAG_TC_I8_ROUTED
 bool mgemm_tc_i8_routed_supported(const DevCtx* ctx, const MGemmArgs& a);
 int launch_mgemm_tc_i8_routed(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a);
+
+// standalone gated activation (act.cu): a = fp16(act(g) * u) elementwise
+int launch_act_mul(cudaStream_t stream, const void* g, const void* u, half* a, long long numel, bool in_fp32, int act, float limit);
 
 int launch_hgemm(cudaStream_t stream, const half* a, const half* b, void* c, int m, int k, int n, bool c_fp32,
                  int64_t c_stride);

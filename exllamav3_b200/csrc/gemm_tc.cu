@@ -23,6 +23,7 @@
 #include "decode.cuh"
 #include "epilogue.cuh"
 #include "f16_pipeline.cuh"
+#include "act.cuh"
 #include <unordered_map>
 #include <mutex>
 
@@ -43,6 +44,22 @@ had_tiled_kernel(const half* __restrict__ A, uint8_t* __restrict__ out, const ha
     if (warp >= m * bpr) return;
     const int r = warp / bpr, kb = warp % bpr;
     uint2 raw = *reinterpret_cast<const uint2*>(A + (size_t) r * k + kb * 128 + lane * 4);
+    if constexpr (HAD) raw = xt_transform(raw, suh + kb * 128 + lane * 4, lane);
+    store_tile_pair(out + (size_t) kb * NT * 256 + xt_tile_offset(r, lane), raw);
+}
+
+// gated variant (exl3b_gemm_gated): the row is fp16(act(G) * U) (act.cuh), then the same transform and tile store
+template <bool HAD>
+__global__ void __launch_bounds__(128)
+had_tiled_gated_kernel(const GateIn gate, uint8_t* __restrict__ out, const half* __restrict__ suh, int m, int k, int NT)
+{
+    pdl_launch_dependents();
+    pdl_wait();
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    const int bpr = k / 128;
+    if (warp >= m * bpr) return;
+    const int r = warp / bpr, kb = warp % bpr;
+    uint2 raw = gated_load4(gate, (size_t) r * k + kb * 128 + lane * 4);
     if constexpr (HAD) raw = xt_transform(raw, suh + kb * 128 + lane * 4, lane);
     store_tile_pair(out + (size_t) kb * NT * 256 + xt_tile_offset(r, lane), raw);
 }
@@ -333,11 +350,17 @@ bool gemm_tc_supported(const GemmArgs& a)
     return a.k >= 128 && a.n >= 128 && a.k % 128 == 0 && a.n % 128 == 0 && a.m >= 1;
 }
 
-static int launch_had_tiled(cudaStream_t stream, const half* A, uint8_t* out, const half* suh, int m, int k, int NT)
+static int launch_had_tiled(cudaStream_t stream, const half* A, uint8_t* out, const half* suh, int m, int k, int NT,
+                            const GateIn* gate)
 {
     const dim3 grid((m * (k / 128) + 3) / 4);
-    const cudaError_t e = suh ? launch_pdl<had_tiled_kernel<true>>(stream, grid, 128, 0, A, out, suh, m, k, NT)
-                              : launch_pdl<had_tiled_kernel<false>>(stream, grid, 128, 0, A, out, suh, m, k, NT);
+    cudaError_t e;
+    if (gate)
+        e = suh ? launch_pdl<had_tiled_gated_kernel<true>>(stream, grid, 128, 0, *gate, out, suh, m, k, NT)
+                : launch_pdl<had_tiled_gated_kernel<false>>(stream, grid, 128, 0, *gate, out, suh, m, k, NT);
+    else
+        e = suh ? launch_pdl<had_tiled_kernel<true>>(stream, grid, 128, 0, A, out, suh, m, k, NT)
+                : launch_pdl<had_tiled_kernel<false>>(stream, grid, 128, 0, A, out, suh, m, k, NT);
     count_launch();
     EXL3B_CUDA(e);
     return 0;
@@ -368,8 +391,9 @@ int plan_gemm_tc(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* 
     return 0;
 }
 
-int launch_gemm_tc(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
+int launch_gemm_tc(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a, const GateIn* gate)
 {
+    EXL3B_CHECK(!gate || a.m <= F16_MAX_ROWS, EXL3B_ERR_UNSUPPORTED, "exl3_gemm_gated: gated input is one pass of rows");
     const size_t esz = a.c_fp32 ? 4 : 2;
     CUtensorMap tmap;
     { int r = get_weight_tmap(a.B, a.k, a.n, a.K, &tmap); if (r) return r; }
@@ -382,7 +406,7 @@ int launch_gemm_tc(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
         const int slot = ctx->next_slot();
         { int r = ensure_xh_tiled(ctx, (size_t) (a.k / 128) * NT * 256); if (r) return r; }
         uint8_t* xh_tiled = ctx->xh_tiled + (size_t) (slot % DevCtx::XH_SLOTS) * ctx->xh_tiled_slot_bytes;
-        { int r = launch_had_tiled(stream, a.A + (size_t) m0 * a.k, xh_tiled, a.suh, m, a.k, NT); if (r) return r; }
+        { int r = launch_had_tiled(stream, a.A + (size_t) m0 * a.k, xh_tiled, a.suh, m, a.k, NT, gate); if (r) return r; }
 
         TcParams p{};
         p.xh_tiled = xh_tiled; p.B = a.B; p.C = (char*) a.C + (size_t) m0 * a.n * esz; p.svh = a.svh;

@@ -11,13 +11,26 @@ gemm_tc_i8_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
     gemm_tc_i8_body<K, MR, false>(p, &tmap_w, nullptr);
 }
 
+// gated input (exl3b_gemm_gated): the rows are fp16(act(G) * U), formed in the prologue; one rows variant (MR = 4), the activation
+// kind and the input dtype are warp-uniform values of `gate`
+template <int K, int MR>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_i8_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w, const GateIn gate)
+{
+    gemm_tc_i8_body<K, MR, false, false, true>(p, &tmap_w, nullptr, nullptr, &gate);
+}
+template <int K, int MR> constexpr void (*i8_plain_kernel)(const TcParams, const CUtensorMap) = gemm_tc_i8_kernel<K, MR>;
+template <int K> constexpr void (*i8_gated_kernel)(const TcParams, const CUtensorMap, const GateIn) = gemm_tc_i8_kernel<K, 4>;
+
 // ---- host side -------------------------------------------------------------------------------------------------------
 
 template <int K>
-static cudaError_t i8_launch(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap)
+static cudaError_t i8_launch(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap,
+                             const GateIn* gate = nullptr)
 {
-    return p.m <= 4 ? launch_pdl<gemm_tc_i8_kernel<K, 4>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap)
-                    : launch_pdl<gemm_tc_i8_kernel<K, 8>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap);
+    if (gate) return launch_pdl<i8_gated_kernel<K>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap, *gate);
+    return p.m <= 4 ? launch_pdl<i8_plain_kernel<K, 4>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap)
+                    : launch_pdl<i8_plain_kernel<K, 8>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap);
 }
 
 // rows 5..8 need the whole transformed activation cached in shared memory (the per-unit digit warps cannot afford eight Hadamards)
@@ -60,8 +73,9 @@ int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPla
     return 0;
 }
 
-int launch_gemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
+int launch_gemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a, const GateIn* gate)
 {
+    EXL3B_CHECK(!gate || a.m <= 4, EXL3B_ERR_UNSUPPORTED, "exl3_gemm_gated (i8): gated input needs m <= 4");
     CUtensorMap tmap;
     { int r = get_weight_tmap(a.B, a.k, a.n, a.K, &tmap); if (r) return r; }
     TcPlan pl;
@@ -75,7 +89,7 @@ int launch_gemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
     p.stages = pl.stages; p.b_bytes = pl.b_bytes; p.b_load_bytes = pl.b_load_bytes;
     const int grid = pl.grid, smem_total = pl.smem_total;
     cudaError_t err = cudaSuccess;
-    EXL3B_DISPATCH_K(a.K, err = i8_launch<KK>(stream, grid, smem_total, p, tmap));
+    EXL3B_DISPATCH_K(a.K, err = i8_launch<KK>(stream, grid, smem_total, p, tmap, gate));
     count_launch();
     EXL3B_CUDA(err);
     EXL3B_CUDA(cudaPeekAtLastError());

@@ -32,6 +32,7 @@
 //   * instantiated for MR = 4 and MR = 8 activation rows (digit tile with one / two row groups); api.cu auto-selects m <= 4
 #pragma once
 #include "i8_pipeline.cuh"
+#include "act.cuh"
 
 namespace exl3b {
 
@@ -49,9 +50,11 @@ __host__ __device__ inline TcSmemLayout i8_smem_layout(int K, int MR, int stages
 // ROUTED = true (gemm_tc_i8_routed.cu): multi-matrix launch whose CTA groups are the ACTIVE SLOTS of an exl3_mgemm call with
 // indices / weights / expert-range filter (MoE decode); slot -> matrix and the slot's output weight come from the table the
 // resolve kernel wrote just before this launch.
-template <int K, int MR, bool AR, bool ROUTED = false>
+// GATED = true (gemm_tc_i8.cu, exl3b_gemm_gated): the rows are fp16(act(G) * U) (act.cuh), formed where the plain kernel loads
+// A_raw; everything from the input transform on is the plain kernel's.
+template <int K, int MR, bool AR, bool ROUTED = false, bool GATED = false>
 __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtensorMap* tmap_w, const ArArgs* ar,
-                                                const RouteArgs* route = nullptr)
+                                                const RouteArgs* route = nullptr, const GateIn* gate = nullptr)
 {
     extern __shared__ __align__(1024) uint8_t smem[];
     constexpr int I8_B_BYTES = i8_b_bytes(MR);
@@ -166,6 +169,14 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     const int ubeg = unit_begin(U, G, cta), uend = unit_begin(U, G, cta + 1);
     const int n_units = uend - ubeg;
 
+    // the raw fp16 inputs k = kb * 128 + 4 lane .. + 3 of row r
+    auto raw_block = [&](int r, int kb) -> uint2
+    {
+        const size_t e = (size_t) r * p.k + kb * 128 + lane * 4;
+        if constexpr (GATED) return gated_load4(*gate, e);
+        else return *reinterpret_cast<const uint2*>(A_raw + e);
+    };
+
     // fp16 transformed activation of (row r, k-block kb), 4 values per lane, exactly as the reference's A_had
     auto xh_finish = [&](uint2 raw, uint2 scb, float (&v)[4])
     {
@@ -183,7 +194,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     };
     auto xh_block = [&](int r, int kb, float (&v)[4])
     {
-        const uint2 raw = *reinterpret_cast<const uint2*>(A_raw + (size_t) r * p.k + kb * 128 + lane * 4);
+        const uint2 raw = raw_block(r, kb);
         uint2 scb = make_uint2(0, 0);
         if (suh) scb = *reinterpret_cast<const uint2*>(suh + kb * 128 + lane * 4);
         xh_finish(raw, scb, v);
@@ -233,9 +244,9 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                     sc0 = *reinterpret_cast<const uint2*>(suh + ka * 128 + lane * 4);
                     if (tb < T) sc1 = *reinterpret_cast<const uint2*>(suh + kb_ * 128 + lane * 4);
                 }
-                const uint2 raw0 = *reinterpret_cast<const uint2*>(A_raw + (size_t) ra * p.k + ka * 128 + lane * 4);
+                const uint2 raw0 = raw_block(ra, ka);
                 uint2 raw1 = make_uint2(0, 0);
-                if (tb < T) raw1 = *reinterpret_cast<const uint2*>(A_raw + (size_t) rb * p.k + kb_ * 128 + lane * 4);
+                if (tb < T) raw1 = raw_block(rb, kb_);
                 float v[4];
                 xh_finish(raw0, sc0, v);
                 xh_publish(ra, ka, v);
@@ -259,7 +270,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                 for (int r = 0; r < MR; ++r)
                 {
                     raw[r] = make_uint2(0, 0);
-                    if (r < p.m) raw[r] = *reinterpret_cast<const uint2*>(A_raw + (size_t) r * p.k + kb * 128 + lane * 4);
+                    if (r < p.m) raw[r] = raw_block(r, kb);
                 }
                 #pragma unroll
                 for (int r = 0; r < MR; ++r)

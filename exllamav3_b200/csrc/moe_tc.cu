@@ -22,6 +22,7 @@
 // read out of the device pointer tables: no tensor map has to be encoded on the host or patched per CTA and fenced when a
 // CTA moves to another expert.
 #include "f16_pipeline.cuh"
+#include "act.cuh"
 #include <mutex>
 #include <vector>
 
@@ -397,15 +398,8 @@ moe_gemm_kernel(const MoeGemmParams p)
 }
 
 // ---- 5. activation into down's input ---------------------------------------------------------------------------------------
-// g, u are fp16 exl3_gemm outputs (output Hadamard and svh applied).  h = fp16(act(g) * u) with the optional clamps
-// u in [-L, L], act(g) <= L; then down's input transform.  ReLU^2 without a gate: act = max(u, 0), taken before the clamp.
-__device__ __forceinline__ float moe_act(float g, float u, int act)
-{
-    if (act == 0) return g / (1.0f + expf(-g));
-    if (act == 1) return 0.5f * g * (1.0f + tanhf(0.797884560803f * (g + 0.044715f * g * g * g)));
-    return fmaxf(u, 0.0f);
-}
-
+// g, u are fp16 exl3_gemm outputs (output Hadamard and svh applied).  h = fp16(act(g) * u) with the limit rule of act.cuh and
+// exl3_moe's own SiLU / GELU expressions (act.cuh); then down's input transform.  ReLU^2 without a gate: act = max(u, 0), taken before the clamp.
 __global__ void __launch_bounds__(128)
 moe_act_kernel(MoeWork w, const half* __restrict__ g, const half* __restrict__ u, const uint64_t* __restrict__ suh_d,
                uint8_t* xd, int N, int k, int act, float limit, int chunk)
@@ -430,10 +424,8 @@ moe_act_kernel(MoeWork w, const half* __restrict__ g, const half* __restrict__ u
     #pragma unroll
     for (int i = 0; i < 4; ++i)
     {
-        float uf = __half2float(uh[i]);
-        float a = moe_act(__half2float(gh[i]), uf, act);
-        if (limit != 0.0f) { uf = fminf(fmaxf(uf, -limit), limit); a = fminf(a, limit); }
-        hv[i] = __float2half_rn(a * uf);
+        const float uf = __half2float(uh[i]), gf = __half2float(gh[i]);
+        hv[i] = act_limit_mul(act == ACT_SILU ? act_silu_moe(gf) : act == ACT_GELU ? act_gelu_moe(gf) : fmaxf(uf, 0.0f), uf, limit);
     }
     uint2 raw;
     raw.x = pack_half2(hv[0], hv[1]); raw.y = pack_half2(hv[2], hv[3]);

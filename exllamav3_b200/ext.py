@@ -10,6 +10,9 @@ behaviour (RuntimeError for shape/dtype violations) as the pybind11 bindings the
     exl3_gemv, g_get_cc, g_get_num_sms, exl3_gemm_num_kernel_shapes, exl3_gemm_shape_compat     bindings.cpp:127-131
     exl3_moe, exl3_moe_max_concurrency         bindings.cpp:209-210
     quantize_tiles, pack_trellis               bindings.cpp:116,119 (the converter's trellis encoder)
+    silu_mul, gelu_mul, relu2_mul              exllamav3_ext/activation.cu (gated activations)
+    BC_GatedMLP, BC_MLP                        exllamav3_ext/libtorch/mlp_bc.h, mlp.cpp (MLP decode blocks)
+    exl3_gemm_gated                            this library's own: the down projection with the activation in its input stage
 
 PyTorch is plumbing only here: device memory, the current CUDA stream and the device guard.
 There is no CPU or torch fallback: if the shared library is missing this module fails to import, and every op
@@ -96,6 +99,8 @@ _lib.exl3b_moe.argtypes = [_vp] * 6 + [_i] * 11 + [_vp] * 9 + [_i] * 6 + [_f, _i
 _lib.exl3b_moe.restype = _i
 _lib.exl3b_moe_max_concurrency.argtypes = [_i]; _lib.exl3b_moe_max_concurrency.restype = _i
 _lib.exl3b_moe_plan.argtypes = [_vp, _i, _i, _i, _i, _i, ctypes.POINTER(MoePlan), _vp, _vp]; _lib.exl3b_moe_plan.restype = _i
+_lib.exl3b_act_mul.argtypes = [_vp] * 4 + [_i64, _i, _i, _f]; _lib.exl3b_act_mul.restype = _i
+_lib.exl3b_gemm_gated.argtypes = [_vp] * 7 + [_i] * 8 + [_f, _i]; _lib.exl3b_gemm_gated.restype = _i
 _lib.exl3b_quantize_tiles.argtypes = [_vp] * 4 + [_i64, _i, _i]; _lib.exl3b_quantize_tiles.restype = _i
 _lib.exl3b_pack_trellis.argtypes = [_vp] * 3 + [_i64, _i]; _lib.exl3b_pack_trellis.restype = _i
 
@@ -109,6 +114,8 @@ EXL3B_TAG_TC_I8_AR = 211
 EXL3B_TAG_TC_I8_ROUTED = 212
 EXL3B_TAG_TC_MOE = 230
 TP_HANDLE_BYTES = 64
+ACT_SILU, ACT_GELU, ACT_RELU2 = 0, 1, 2
+MAX_BSZN = 8        # rows of BC_GatedMLP.run_bszN, as the reference's modules/mlp.py MAX_BSZN
 
 lib = _lib      # raw handle for bench.py / tests (symbol export checks)
 lib_path = _LIB_PATH
@@ -719,6 +726,180 @@ class BC_LinearEXL3:
             return y
         self.run(x.view(-1, x.shape[-1]), y.view(-1, out_features))
         return y
+
+
+# ---- gated activations and the MLP blocks (exllamav3_ext/activation.cu, libtorch/mlp.cpp) ------------------------------------
+
+def _act_mul(act: int, name: str, x, y, z, act_limit: float) -> None:
+    _need_cuda(x, y, z)
+    if x.dtype == torch.float:
+        _dtype(y, torch.float, "y")
+    else:
+        _dtype(x, torch.half, "x")
+        _dtype(y, torch.half, "y")
+    _dtype(z, torch.half, "z")
+    if y.numel() != x.numel() or z.numel() != x.numel():
+        raise RuntimeError(f"{name}: x, y and z must have the same number of elements")
+    if not (x.is_contiguous() and y.is_contiguous() and z.is_contiguous()):
+        raise RuntimeError(f"{name}: x, y and z must be contiguous")
+    if y.device != x.device or z.device != x.device:
+        raise RuntimeError(f"{name}: x, y and z must be on one device")
+    with torch.cuda.device(x.device):
+        _check(_lib.exl3b_act_mul(_stream(x), _ptr(x), _ptr(y), _ptr(z), x.numel(), int(x.dtype == torch.float), act,
+                                  float(act_limit)))
+
+
+def silu_mul(x, y, z, act_limit: float) -> None:
+    """
+    z = silu(x) * y, with the limit rule of the reference (act_limit != 0: y clamped to [-act_limit, act_limit], silu(x) from above
+    at act_limit).  x, y fp16 or both fp32, z fp16, equal element counts, contiguous; z may be x or y.  exllamav3_ext/activation.cu.
+    Computed in fp32 and rounded to fp16 once; the reference's fp16-input kernel computes in half arithmetic (h2exp, h2rcp), so
+    results can differ from it in the last bit.
+    """
+    _act_mul(ACT_SILU, "silu_mul", x, y, z, act_limit)
+
+
+def gelu_mul(x, y, z, act_limit: float) -> None:
+    """z = gelu(x) * y, gelu in the tanh form; otherwise as silu_mul (fp32 arithmetic, one rounding)."""
+    _act_mul(ACT_GELU, "gelu_mul", x, y, z, act_limit)
+
+
+def relu2_mul(x, y, z, act_limit: float) -> None:
+    """z = max(x, 0)^2 * y; otherwise as silu_mul (fp32 arithmetic, one rounding)."""
+    _act_mul(ACT_RELU2, "relu2_mul", x, y, z, act_limit)
+
+
+def exl3_gemm_gated(G, U, B, C, suh, svh, act: int, act_limit: float, mcg, mul1, force_num_sms: int = 0) -> int:
+    """
+    exl3_gemm(act_mul(G, U), B, C, suh, svh) without the intermediate: the kernel forms fp16(act(G) * U) where it reads its input
+    rows.  G, U (m, k) fp16 or both fp32, contiguous, m <= 8 (e.g. the two halves of a (2, m, k) exl3_mgemm output); act is
+    ACT_SILU, ACT_GELU or ACT_RELU2.  Bit-identical to silu_mul / gelu_mul / relu2_mul into a buffer followed by exl3_gemm on it,
+    on the same path and grid: tag 210 for mul1 at m <= 4, tag 200 otherwise (include/exl3b200.h).  Returns the path tag.
+    """
+    _need_cuda(G, U, B, C, suh, svh)
+    if B.dim() != 3:
+        raise RuntimeError("B: incorrect number of dimensions, must be 3")
+    _dtype(B, torch.int16, "B")
+    if G.dtype == torch.float:
+        _dtype(U, torch.float, "U")
+    else:
+        _dtype(G, torch.half, "G")
+        _dtype(U, torch.half, "U")
+    c_fp32 = C.dtype == torch.float
+    if not c_fp32:
+        _dtype(C, torch.half, "C")
+    size_k = G.shape[-1]
+    size_m = G.numel() // size_k if size_k else 0
+    size_n = B.shape[1] * 16
+    if U.shape != G.shape:
+        raise RuntimeError("G and U incompatible shapes")
+    if size_k != B.shape[0] * 16:
+        raise RuntimeError("G and B incompatible shapes")
+    if C.shape[-1] != size_n or C.numel() != size_m * size_n:
+        raise RuntimeError("C and B incompatible shapes")
+    if not (G.is_contiguous() and U.is_contiguous() and B.is_contiguous() and C.is_contiguous()):
+        raise RuntimeError("exl3_gemm_gated: tensors must be contiguous")
+    K = B.shape[2] // 16
+    with torch.cuda.device(G.device):
+        return _check(_lib.exl3b_gemm_gated(
+            _stream(G), _ptr(G), _ptr(U), _ptr(B), _ptr(C), _ptr(suh), _ptr(svh), size_m, size_k, size_n, K, _cb(mcg, mul1),
+            int(c_fp32), int(G.dtype == torch.float), int(act), float(act_limit), int(force_num_sms)))
+
+
+def _act_kind(act_silu: bool, act_gelu: bool, act_relu2: bool, name: str) -> int:
+    if act_silu:
+        return ACT_SILU
+    if act_gelu:
+        return ACT_GELU
+    if act_relu2:
+        return ACT_RELU2
+    raise RuntimeError(f"{name}: one of act_silu, act_gelu, act_relu2 must be set")
+
+
+class BC_GatedMLP:
+    """
+    Gated MLP decode block, exllamav3_ext/libtorch/mlp_bc.h and mlp.cpp (same constructor arguments, so modules/mlp.py binds it
+    unchanged).  run_bszN(x, d) for 1..MAX_BSZN tokens is two launches where the reference issues three: gate and up (one
+    exl3_mgemm over the pointer tables, or two exl3_gemm on the `gate` / `up` BC_LinearEXL3 plus their biases), then
+    exl3_gemm_gated for down, which applies the activation in its input stage, then down's bias.  Results are bit-identical to
+    exl3_mgemm -> silu_mul / gelu_mul / relu2_mul -> exl3_gemm on this library.
+    `a` and `down_xh` are accepted and left untouched: the activated intermediate is never written (as A_had elsewhere, the
+    library keeps its own scratch).  `guh` / `gu` give width and dtype; the gate/up outputs go to exactly shaped (2, tokens, width)
+    buffers kept per token count (the mgemm slot stride is tokens * width, libtorch/mlp.cpp:22-26).
+    Runs eagerly on the current stream; a caller may capture it in a CUDA graph after one eager call per token count.
+    """
+
+    def __init__(self, guh, gu, a, down_xh, gu_ptrs_trellis, gu_ptrs_suh, gu_ptrs_svh, gu_K: int, gu_mcg: bool, gu_mul1: bool,
+                 act_silu: bool, act_gelu: bool, act_relu2: bool, gate, up, down, act_limit: float):
+        self.act = _act_kind(act_silu, act_gelu, act_relu2, "BC_GatedMLP")
+        if gu_ptrs_trellis is None and (gate is None or up is None):
+            raise RuntimeError("BC_GatedMLP: needs the gate/up pointer tables or the gate and up linears")
+        self.guh, self.gu, self.a, self.down_xh = guh, gu, a, down_xh
+        self.gu_ptrs_trellis, self.gu_ptrs_suh, self.gu_ptrs_svh = gu_ptrs_trellis, gu_ptrs_suh, gu_ptrs_svh
+        self.gu_K, self.gu_mcg, self.gu_mul1 = int(gu_K), bool(gu_mcg), bool(gu_mul1)
+        self.gate, self.up, self.down, self.act_limit = gate, up, down, float(act_limit)
+        self._bufs = {}
+
+    def _buffers(self, num_tokens: int):
+        b = self._bufs.get(num_tokens)
+        if b is None:
+            b = (torch.empty((2, num_tokens, self.guh.shape[2]), dtype=self.guh.dtype, device=self.guh.device),
+                 torch.empty((2, num_tokens, self.gu.shape[2]), dtype=self.gu.dtype, device=self.gu.device))
+            self._bufs[num_tokens] = b
+        return b
+
+    def run_bszN(self, x, d) -> None:
+        num_tokens = x.numel() // x.shape[-1] if x.shape[-1] else 0
+        if not 1 <= num_tokens <= MAX_BSZN:
+            raise RuntimeError("run_bszN: bsz out of supported range")
+        guh_n, gu_n = self._buffers(num_tokens)
+        x3 = x.view(1, num_tokens, x.shape[-1])
+        g, u = gu_n[0], gu_n[1]
+        if self.gu_ptrs_trellis is not None:
+            exl3_mgemm(x3, self.gu_ptrs_trellis, gu_n, self.gu_ptrs_suh, guh_n, self.gu_ptrs_svh, None, None, self.gu_K, -1,
+                       self.gu_mcg, self.gu_mul1, -1, -1, 0)
+        else:
+            gt, up = self.gate, self.up
+            exl3_gemm(x3, gt.trellis, g, gt.suh, guh_n[0], gt.svh, -1, gt.mcg, gt.mul1, 0)
+            exl3_gemm(x3, up.trellis, u, up.suh, guh_n[1], up.svh, -1, up.mcg, up.mul1, 0)
+            if gt.bias is not None:
+                g += gt.bias
+            if up.bias is not None:
+                u += up.bias
+        dn = self.down
+        exl3_gemm_gated(g, u, dn.trellis, d, dn.suh, dn.svh, self.act, self.act_limit, dn.mcg, dn.mul1)
+        if dn.bias is not None:
+            d += dn.bias
+
+
+class BC_MLP:
+    """
+    Ungated MLP decode block for one token, exllamav3_ext/libtorch/mlp_bc.h and mlp.cpp (same constructor arguments, so
+    modules/mlp.py binds it unchanged).  run_bsz1(x, d): the optional zero-padded staging copy into `xp`, up (with its bias)
+    into `u`, then down as exl3_gemm_gated(G = u, U = ones) -- the reference's in-place act_mul(u, ones, u) applied in down's input
+    stage, so `u` keeps up's output -- then down's bias, and the optional copy out of the padded `yp`.  Runs eagerly.
+    """
+
+    def __init__(self, xp, u, ones, yp, act_silu: bool, act_gelu: bool, act_relu2: bool, up, down, act_limit: float,
+                 hidden_size: int, out_size: int):
+        self.act = _act_kind(act_silu, act_gelu, act_relu2, "BC_MLP")
+        self.xp, self.u, self.ones, self.yp = xp, u, ones, yp
+        self.up, self.down, self.act_limit = up, down, float(act_limit)
+        self.hidden_size, self.out_size = int(hidden_size), int(out_size)
+
+    def run_bsz1(self, x, d) -> None:
+        x_in = x
+        if self.xp is not None:
+            self.xp[:, :self.hidden_size].copy_(x.view(1, self.hidden_size))
+            x_in = self.xp.view(1, 1, -1)
+        self.up.run(x_in.view(1, -1), self.u.view(1, -1))
+        dn = self.down
+        y = self.yp.view(1, 1, -1) if self.yp is not None else d
+        exl3_gemm_gated(self.u, self.ones, dn.trellis, y, dn.suh, dn.svh, self.act, self.act_limit, dn.mcg, dn.mul1)
+        if dn.bias is not None:
+            y += dn.bias
+        if self.yp is not None:
+            d.view(1, self.out_size).copy_(self.yp[:, :self.out_size])
 
 
 # ---- trellis encoder (the converter's two GPU bindings, modules/quant/exl3_lib/quantize.py) ---------------------------------

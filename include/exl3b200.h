@@ -125,6 +125,31 @@ int exl3b_gemm(void* stream,
                int force_shape_idx, int force_num_sms);
 
 /*
+ * exl3b_act_mul -- replaces ext.silu_mul / gelu_mul / relu2_mul (exllamav3_ext/activation.cu).
+ *
+ *   a[i] = fp16( act(g[i]) * u[i] ),   act = 0 SiLU g / (1 + exp(-g)), 1 GELU (tanh form), 2 ReLU^2 max(g, 0)^2
+ *   act_limit != 0: u is clamped to [-act_limit, act_limit] and act(g) from above at act_limit first.
+ *
+ *   g, u   numel elements, fp16 (in_fp32 = 0) or fp32 (in_fp32 = 1), contiguous; a numel fp16, may alias g or u.
+ *   Computed in fp32 and rounded once (the reference's fp16-input kernel computes in half arithmetic).  Returns 0.
+ */
+int exl3b_act_mul(void* stream, const void* g, const void* u, void* a, int64_t numel, int in_fp32, int act, float act_limit);
+
+/*
+ * exl3b_gemm_gated -- exl3b_gemm(exl3b_act_mul(G, U), B, ...) with the activation applied where the GEMM reads its input: the
+ * down projection of a gated MLP block without the intermediate tensor.  Bit-identical to exl3b_act_mul into a buffer followed by
+ * exl3b_gemm on it, with the same path and grid.
+ *
+ *   G, U   (m, k) fp16 (gu_fp32 = 0, 8-byte aligned) or fp32 (gu_fp32 = 1, 16-byte aligned), contiguous; e.g. the gate and up
+ *          rows of an exl3b_mgemm output (2, m, k)
+ *   B, C, suh, svh, K, cb, c_fp32, force_num_sms   as exl3b_gemm;  act, act_limit   as exl3b_act_mul
+ *   Paths: the one exl3b_gemm selects for (m, k, n, K, cb) under exl3b_set_gemm_path, when it is EXL3B_TAG_TC_I8 at m <= 4 or
+ *   EXL3B_TAG_TC at m <= 8.  Any other selection, and m > 8, returns -EXL3B_ERR_UNSUPPORTED.  Returns the path tag.
+ */
+int exl3b_gemm_gated(void* stream, const void* G, const void* U, const void* B, void* C, const void* suh, const void* svh,
+                     int m, int k, int n, int K, int cb, int c_fp32, int gu_fp32, int act, float act_limit, int force_num_sms);
+
+/*
  * exl3b_mgemm -- replaces ext.exl3_mgemm (exllamav3_ext/bindings.cpp:146, exllamav3_ext/quant/exl3_gemm.cuh:58-78; semantics
  * exllamav3_ext/quant/exl3_gemm.cu:341-381).
  *
