@@ -8,7 +8,8 @@ chunks.  Whether a shape reaches a branch is decided by the host planner (exl3b_
 row of those tables still hits the regime it is there for.  A planner change that shrinks the coverage fails here instead of
 letting the GPU tests pass without testing anything.
 
-It also owns what both files share: the tables, the worst-case int32 input and the plan helpers.
+It also owns what both files share: the tables, the worst-case int32 input and the plan helpers, and the checker of the fp16
+paths (tags 100 and 200, exl3_moe) against their exact models, with its bars, which every GPU file that reaches those paths uses.
 """
 import ctypes
 import numpy as np
@@ -105,6 +106,64 @@ def worst_case_inputs(m, k=WORST_K, n=WORST_N, K=WORST_KQ, s0=0.5):
     x = np.zeros((m, k), dtype=np.float16)
     x[:, ::128] = 1.0
     return tr, suh, svh, x
+
+
+# ---- the fp16 paths against their exact models -----------------------------------------------------------------------------
+# oracle.exl3_gemm_f16_model / exl3_mgemm_f16_model / exl3_moe_model are these paths' arithmetic up to the order of the fp32
+# accumulation (README.md, Parity).  The kernels accumulate in fp32 along k, so their distance to the model grows like
+# 2^-24 sqrt(k) max|y|: measured on an H100 (80 GB HBM3, 700 W) over the GPU suite, fp32 C is at most 5.0e-6 max|y| max-abs and
+# 4.3e-6 rel-RMS from the model (k = 14336, tag 200; 3e-7 at k = 512).
+#   fp32 C: max-abs / max|y| and rel-RMS <= F16_MODEL_BAR, the int8 paths' bars.
+#   fp16 C: every element within F16_MODEL_STEPS x oracle.f16_model_tol of the model (roundings of the pre-svh value and of C
+#           that went the other way) plus F16_MODEL_BAR[0] max|y| (the accumulation order, as for fp32 C), and at least
+#           F16_MODEL_SAME of the elements bit-identical to the model.  Measured: at most 1.0 x f16_model_tol + 2e-5 max|y| (tag 100);
+#           1.9 % of the elements differ at k = 14336 (4096 x 14336 down, 32 rows), 0.5 % at k = 512.  svh applied in fp32
+#           before the one fp16 rounding changes 26 %.
+#   exl3_moe: the same accumulation noise flips ~2 % of the fp16 roundings of g and u, and so of h, before the down projection;
+#           measured at most 3.4e-4 max-abs and 1.6e-4 rel-RMS from exl3_moe_model (Mixtral widths, several chunks).
+F16_MODEL_BAR = (2e-5, 1e-5)
+F16_MODEL_SAME = 0.925
+F16_MODEL_STEPS = 4
+MOE_MODEL_BAR = (1.4e-3, 6.5e-4)
+
+
+def rel_err(y, ref):
+    y = np.asarray(y, dtype=np.float64); ref = np.asarray(ref, dtype=np.float64)
+    err = np.abs(y - ref)
+    return err.max() / max(np.abs(ref).max(), 1e-30), np.sqrt((err ** 2).mean()) / max(np.sqrt((ref ** 2).mean()), 1e-30)
+
+
+def f16_model_ratios(y, model, tol):
+    """fp16 C against its model: (largest |y - model| over its bound, share of elements that are not bit-identical)."""
+    y64, m64 = np.asarray(y, dtype=np.float64), np.asarray(model, dtype=np.float64)
+    bound = F16_MODEL_STEPS * tol + F16_MODEL_BAR[0] * np.abs(m64).max()
+    d = np.abs(y64 - m64)
+    worst = float(np.max(np.where(d > 0, d / np.maximum(bound, 1e-300), 0.0)))
+    return worst, float((np.asarray(y, dtype=np.float16) != np.asarray(model, dtype=np.float16)).mean())
+
+
+def check_f16_model(y, model, tol, what, bar=F16_MODEL_BAR):
+    """
+    C of an fp16-path call against its model.  tol None: fp32 C, held to `bar`; else fp16 C, held element-wise to
+    F16_MODEL_STEPS x tol (f16_model_tol, or the mgemm model's sum of it) plus F16_MODEL_BAR[0] max|y|, and to F16_MODEL_SAME
+    bit-identical elements.
+    """
+    if tol is None:
+        mx, rms = rel_err(y, model)
+        assert mx <= bar[0] and rms <= bar[1], ("fp16-path model", what, mx, rms)
+        return
+    worst, changed = f16_model_ratios(y, model, tol)
+    assert worst <= 1.0 and changed <= 1 - F16_MODEL_SAME, ("fp16-path model, fp16 C", what, worst, changed)
+
+
+def check_f16_gemm(y, x, tr, suh, svh, K, cb, fp32, what, w=None):
+    """One exl3_gemm call on tag 100 or 200 (C as float64 or its own dtype) against oracle.exl3_gemm_f16_model."""
+    model, pre = orc.exl3_gemm_f16_model(x, tr, suh, svh, K, cb, np.float32 if fp32 else np.float16, w=w)
+    check_f16_model(y, model, None if fp32 else orc.f16_model_tol(model, pre, svh), what)
+
+
+def check_moe_model(y, model, what):
+    check_f16_model(y, model, None, what, MOE_MODEL_BAR)
 
 
 # ---- tests -----------------------------------------------------------------------------------------------------------

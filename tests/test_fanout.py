@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 from oracle import exl3_oracle as orc
+from test_edges_host import check_f16_gemm
 
 
 def test_fanout_partition_properties():
@@ -203,6 +204,9 @@ def test_fanout_fallbacks_and_rewritten_width_list(cuda):
             ref = orc.exl3_gemm_f64(x[0].cpu().numpy(), tr.cpu().numpy(), suh.cpu().numpy(), svh.cpu().numpy(), K, 2)
             mx, rms = rel(o.float().cpu().numpy(), ref)
             assert mx <= 4e-3 + 2.0 ** -10 and rms <= 2e-3, (widths, mx, rms)
+            if tag in (ext.EXL3B_TAG_SIMT, ext.EXL3B_TAG_TC):             # the generic path: fp16 C of the exact model
+                check_f16_gemm(o.cpu().numpy(), x[0].cpu().numpy(), tr.cpu().numpy(), suh.cpu().numpy(), svh.cpu().numpy(), K, 2,
+                               False, (widths, tag))
         return keep
 
     check([128, 256] * 4 + [128], expect_tc=False)       # nine matrices: generic path

@@ -9,14 +9,15 @@ Every call writes into the middle rows of a larger C filled with a sentinel bit 
 trailing rows are NaN: the rows around the output must keep their bits and every valid output must stay finite.
 
 Bars (README.md, Parity): vs oracle.exl3_gemm_f64 max-abs <= 2e-3 max|y| (+1 fp16 ulp), rel-RMS <= 1e-3; the int8 path vs its
-exact model oracle.exl3_gemm_i8_model max-abs <= 2e-5 max|y|, rel-RMS <= 1e-5 (fp32 C), 1.5e-3 / 5e-4 (fp16 C).
+exact model oracle.exl3_gemm_i8_model max-abs <= 2e-5 max|y|, rel-RMS <= 1e-5 (fp32 C), 1.5e-3 / 5e-4 (fp16 C); tags 100 and 200
+vs their exact model oracle.exl3_gemm_f16_model with test_edges_host.check_f16_gemm.
 """
 import contextlib
 import numpy as np
 import pytest
 import torch
 from oracle import exl3_oracle as orc
-from test_edges_host import CACHE_PAIRS, FORCED_GRIDS, WORST_KQ, gemm_plan, worst_case_inputs
+from test_edges_host import CACHE_PAIRS, FORCED_GRIDS, WORST_KQ, check_f16_gemm, gemm_plan, worst_case_inputs
 
 pytestmark = pytest.mark.gpu
 
@@ -115,6 +116,7 @@ def test_every_instantiation(cuda, K, cb, path):
                     y, tag = run(ext, cuda, x[:m], mt, fp32)
                     assert tag == path
                     check_f64(y, ref, fp32, (K, cb, k, n, m))
+                    check_f16_gemm(y, x[:m], tr, suh, svh, K, cb, fp32, (K, cb, k, n, m), w=w)
 
 
 _RECON_HAD_COVERED = {(1, 0), (2, 1), (3, 2), (4, 2), (5, 0), (6, 2), (7, 1), (8, 2)}       # test_gpu_parity.py
@@ -167,6 +169,7 @@ def test_row_sweep_exact_path(cuda, K, cb):
                 y, tag = run(ext, cuda, x[:m], mt, fp32)
                 assert tag == TAG_TC
                 check_f64(y, ref, fp32, (K, cb, m))
+                check_f16_gemm(y, x[:m], tr, suh, svh, K, cb, fp32, (K, cb, m), w=w)
 
 
 def test_canaries_int8_and_cuda_core_paths(cuda):
@@ -194,6 +197,7 @@ def test_canaries_int8_and_cuda_core_paths(cuda):
                 y, tag = run(ext, cuda, x[:m], mt, fp32)
                 assert tag == TAG_SIMT
                 check_f64(y, ref, fp32, m)
+                check_f16_gemm(y, x[:m], tr, suh, svh, 3, 0, fp32, m, w=w)
 
 
 # ---- 3. forced persistent grids ------------------------------------------------------------------------------------------
@@ -214,10 +218,12 @@ def test_forced_grids_exact_path(cuda, k, n, grids):
                     y, tag = run(ext, cuda, x[:m], mt, False, force=G)
                     assert tag == TAG_TC
                     check_f64(y, ref, False, (cb, m, G))
+                    check_f16_gemm(y, x[:m], tr, suh, svh, 4, cb, False, (cb, m, G), w=w)
                     y1, _ = run(ext, cuda, x[:m], mt, True, force=G)
                     y2, _ = run(ext, cuda, x[:m], mt, True, force=G)
                     assert np.array_equal(y1, y2), (cb, m, G)
                     check_f64(y1, ref, True, (cb, m, G))
+                    check_f16_gemm(y1, x[:m], tr, suh, svh, 4, cb, True, (cb, m, G), w=w)
 
 
 @pytest.mark.parametrize("k,n,grids", FORCED_GRIDS)
@@ -382,3 +388,6 @@ def test_graph_replay_matches_eager(cuda):
             y, tag = run(ext, cuda, c["xs"][rnd], c["mt"], True)
             assert tag == c["tag"]
             assert np.array_equal(got.double().cpu().numpy(), y), (rnd, c["tag"], c["xs"][0].shape)
+            if c["tag"] == TAG_TC:
+                mt = c["mt"]
+                check_f16_gemm(y, c["xs"][rnd], mt.tr, mt.suh, mt.svh, 4, 2, True, ("replay", rnd))

@@ -7,12 +7,14 @@ the dense wgmma GEMM at 8192 x 4096 x 14336.
 
 Method at sizes the fp64 oracle cannot afford in full: random 128-column blocks of the output against the oracle restricted to
 those columns (a 128-column block of an EXL3 linear is itself a complete EXL3 linear: trellis[:, 8b:8b+8], svh[128b:128b+128]),
-tolerances of README.md, Parity (max-abs <= 2e-3 max|y| (+1 fp16 ulp), rel-RMS <= 1e-3).
+tolerances of README.md, Parity (max-abs <= 2e-3 max|y| (+1 fp16 ulp), rel-RMS <= 1e-3); blocks of calls that ran on tags 100 / 200
+are also held to their exact model (test_edges_host.check_f16_gemm).
 """
 import numpy as np
 import pytest
 import torch
 from oracle import exl3_oracle as orc
+from test_edges_host import check_f16_gemm
 
 pytestmark = pytest.mark.gpu
 
@@ -37,15 +39,21 @@ def synth_gpu(k, n, K, dev, seed):
     return tr, suh, svh
 
 
-def check_blocks(y, x_np, tr, suh, svh, K, cb, blocks, tol=(2e-3, 1e-3), tag=""):
+def check_blocks(y, x_np, tr, suh, svh, K, cb, blocks, tol=(2e-3, 1e-3), tag="", path=None):
+    """path: the call's returned path tag; on tags 100 and 200 each block is also held to the exact model."""
     suh_np = suh.cpu().numpy()
     for blk in blocks:
         sl = slice(blk * 128, blk * 128 + 128)
         tr_b = tr[:, blk * 8: blk * 8 + 8, :].contiguous().cpu().numpy()
-        ref = orc.exl3_gemm_f64(x_np, tr_b, suh_np, svh[sl].cpu().numpy(), K, cb)
-        mx, rms = rel_err(y[..., sl].float().cpu().numpy().reshape(ref.shape), ref)
+        svh_b = svh[sl].cpu().numpy()
+        w = orc.reconstruct(tr_b, K, cb)
+        ref = orc.exl3_gemm_f64(x_np, tr_b, suh_np, svh_b, K, cb, w=w)
+        got = y[..., sl].float().cpu().numpy().reshape(ref.shape)
+        mx, rms = rel_err(got, ref)
         ulp = 2.0 ** -10 if y.dtype == torch.half else 0.0
         assert mx <= tol[0] + ulp and rms <= tol[1], (tag, blk, mx, rms)
+        if path in (100, 200):
+            check_f16_gemm(got, x_np, tr_b, suh_np, svh_b, K, cb, y.dtype == torch.float, (tag, blk), w=w)
 
 
 def run_default(ext, x, tr, suh, svh, fp32=True, mul1=True, mcg=False):
@@ -86,7 +94,8 @@ def test_llama_shapes_other_bitrates(cuda, K, shape):
     for (mcg, cb) in ((False, 0), (True, 1)):
         y, tag = run_default(ext, x, tr, suh, svh, True, mul1=False, mcg=mcg)
         assert tag == ext.EXL3B_TAG_TC
-        check_blocks(y, x.cpu().numpy(), tr, suh, svh, K, cb, rng.choice(n // 128, 2, replace=False), tag=f"{shape} K={K} cb={cb}")
+        check_blocks(y, x.cpu().numpy(), tr, suh, svh, K, cb, rng.choice(n // 128, 2, replace=False), tag=f"{shape} K={K} cb={cb}",
+                     path=tag)
 
 
 @pytest.mark.parametrize("m", [8, 32])
@@ -103,7 +112,7 @@ def test_llama_shapes_batch_8_and_32(cuda, m, shape):
     for fp32 in (True, False):
         y, tag = run_default(ext, x, tr, suh, svh, fp32)
         assert tag != ext.EXL3B_TAG_SIMT                              # batch 8 / 32 runs on the tensor cores
-        check_blocks(y, x.cpu().numpy(), tr, suh, svh, K, 2, rng.choice(n // 128, 2, replace=False), tag=f"{shape} m={m}")
+        check_blocks(y, x.cpu().numpy(), tr, suh, svh, K, 2, rng.choice(n // 128, 2, replace=False), tag=f"{shape} m={m}", path=tag)
 
 
 # Llama-3.1-70B shards as modules/quant/exl3.py:284-330 cuts them (hidden 8192, intermediate 28672, kv 1024):
@@ -156,7 +165,8 @@ def test_dense_mgemm_batch_8_and_32_default_path(cuda, m):
             torch.cuda.synchronize()
             assert tag != ext.EXL3B_TAG_SIMT, "dense multi-matrix calls up to 32 rows must run on the tensor cores"
             for j, (tr, suh, svh) in enumerate(ts):
-                check_blocks(C[j], x[0].cpu().numpy(), tr, suh, svh, K, 2, rng.choice(n // 128, 2, replace=False), tag=f"mgemm m={m} mat {j}")
+                check_blocks(C[j], x[0].cpu().numpy(), tr, suh, svh, K, 2, rng.choice(n // 128, 2, replace=False), tag=f"mgemm m={m} mat {j}",
+                             path=tag)
 
 
 @pytest.mark.parametrize("m", [1, 5])

@@ -6,6 +6,7 @@ CPU oracle on the same seeded inputs, against the committed golden outputs of th
 Tolerances (stated per north_star):
   reconstruct, had_r_128 (fp16 and fp32)   : bit-exact
   exl3_gemm / exl3_mgemm vs fp64 oracle    : max-abs <= 2e-3 * max|y| + 1 output ulp,  rel-RMS <= 1e-3
+  tags 100 / 200 vs their exact model      : test_edges_host.check_f16_model (oracle.exl3_gemm_f16_model, exl3_mgemm_f16_model)
   exl3_gemm vs reference exl3_gemm (golden): max-abs <= 4e-3 * max|y|,  rel-RMS <= 2e-3 (the reference carries fp16
                                              split-K partial rounding, exl3_gemm_inner.cuh:501-503)
   reconstruct_had vs fp64                  : max-abs <= 2e-3 * max|W|   (reference test: tests/test_reconstruct_had.py:56-58)
@@ -18,6 +19,7 @@ import torch
 from conftest import GOLDEN
 from oracle import exl3_oracle as orc
 from oracle import gen_golden_gpu as gg
+from test_edges_host import check_f16_gemm, check_f16_model
 
 pytestmark = pytest.mark.gpu
 
@@ -120,6 +122,7 @@ def test_gemm_vs_oracle(cuda, gemm_path, K, cb, m):
         ulp = 2.0 ** -10 if not fp32 else 0.0
         assert mx <= 2e-3 + ulp, (K, cb, m, fp32, mx)
         assert rms <= 1e-3, (K, cb, m, fp32, rms)
+        check_f16_gemm(y, x, tr, suh, svh, K, cb, fp32, (gemm_path, K, cb, m))
 
 
 def test_gemm_without_scratch_and_ragged_rows(cuda, gemm_path):
@@ -128,15 +131,19 @@ def test_gemm_without_scratch_and_ragged_rows(cuda, gemm_path):
     for m in (1, 3, 8, 9, 31, 33, 144, 300):          # rows up to the reconstruct threshold (modules/quant/exl3.py:10)
         tr, suh, svh, x = orc.make_synthetic(k, n, K, m=m)
         ref = orc.exl3_gemm_f64(x, tr, suh, svh, K, cb)
-        y, _, _ = run_gemm(ext, cuda, x, tr, suh, svh, K, cb, True, a_had=False)
+        y, _, tag = run_gemm(ext, cuda, x, tr, suh, svh, K, cb, True, a_had=False)
         mx, rms = rel_err(y, ref)
         assert mx <= 2e-3 and rms <= 1e-3, (m, mx, rms)
+        if tag in (ext.EXL3B_TAG_SIMT, ext.EXL3B_TAG_TC):
+            check_f16_gemm(y, x, tr, suh, svh, K, cb, True, (gemm_path, m))
     # A_had aliasing A is allowed (science/qgemm_benchmark.py:85)
     tr, suh, svh, x = orc.make_synthetic(k, n, K, m=4)
     A = T(x, cuda); C = torch.empty((4, n), dtype=torch.half, device=cuda)
-    ext.exl3_gemm(A, T(tr, cuda), C, T(suh, cuda), A, T(svh, cuda), -1, False, True, 0)
+    tag = ext.exl3_gemm(A, T(tr, cuda), C, T(suh, cuda), A, T(svh, cuda), -1, False, True, 0)
     mx, rms = rel_err(C.cpu().numpy(), orc.exl3_gemm_f64(x, tr, suh, svh, K, cb))
     assert mx <= 3e-3 and rms <= 1e-3
+    if tag in (ext.EXL3B_TAG_SIMT, ext.EXL3B_TAG_TC):
+        check_f16_gemm(C.cpu().numpy(), x, tr, suh, svh, K, cb, False, (gemm_path, "aliased A_had"))
 
 
 def test_gemm_vs_reference_cuda_golden(cuda, gemm_path):
@@ -306,6 +313,8 @@ def test_linear_exl3_kernel_vs_reconstruct_path(cuda):
 
 
 def test_mgemm_modes(cuda):
+    """The four modes of exl3_mgemm on the default path and on the CUDA-core kernels (tag 100), which are also held to their
+    exact model."""
     from exllamav3_b200 import ext, QLinear, pointer_tables
     from types import SimpleNamespace
     k, n, K, m, mats, A, wts = gg.mgemm_inputs()
@@ -314,46 +323,64 @@ def test_mgemm_modes(cuda):
     ml = SimpleNamespace(ptrs_trellis=pt[0], ptrs_suh=pt[1], ptrs_svh=pt[2], mcg=False, mul1=True)
     trs = [t[0] for t in mats]; suhs = [t[1] for t in mats]; svhs = [t[2] for t in mats]
     golden = np.load(os.path.join(GOLDEN, "ref_gpu.npz")) if os.path.exists(os.path.join(GOLDEN, "ref_gpu.npz")) else None
-    for fp32 in (False, True):
-        dt = torch.float if fp32 else torch.half
-        npdt = np.float32 if fp32 else np.float16
-        Ah = torch.empty((4, m, k), dtype=torch.half, device=cuda)
-        tol = 3e-3
-        # (a) one input, four outputs
-        C = torch.zeros((4, m, n), dtype=dt, device=cuda)
-        ext.exl3_mgemm(T(A[:1], cuda), ml.ptrs_trellis, C, ml.ptrs_suh, Ah, ml.ptrs_svh, None, None, K, -1,
-                       ml.mcg, ml.mul1, -1, -1, 0)
-        ref = orc.exl3_mgemm(A[:1], trs, suhs, svhs, K, 2, npdt, bszm_out=4)
-        assert rel_err(C.cpu().numpy(), ref)[0] <= tol
-        if golden is not None:
-            assert rel_err(C.cpu().numpy(), golden[f"mgemm_a_{int(fp32)}"])[0] <= 5e-3
-        # (b) indices with a skipped slot
-        C = torch.zeros((4, m, n), dtype=dt, device=cuda)
-        idx = torch.tensor([[2, -1, 0, 3]], dtype=torch.long, device=cuda)
-        ext.exl3_mgemm(T(A, cuda), ml.ptrs_trellis, C, ml.ptrs_suh, Ah, ml.ptrs_svh, idx, None, K, -1,
-                       ml.mcg, ml.mul1, -1, -1, 0)
-        ref = orc.exl3_mgemm(A, trs, suhs, svhs, K, 2, npdt, indices=[2, -1, 0, 3], bszm_out=4)
-        assert rel_err(C.cpu().numpy(), ref)[0] <= tol and float(C[1].abs().max()) == 0.0
-        if golden is not None:
-            assert rel_err(C.cpu().numpy(), golden[f"mgemm_b_{int(fp32)}"])[0] <= 5e-3
-        # (c) weighted reduction into C[0]
-        C = torch.zeros((4, m, n), dtype=dt, device=cuda)
-        idx = torch.tensor([[3, 1, 0, 2]], dtype=torch.long, device=cuda)
-        ext.exl3_mgemm(T(A[:1], cuda), ml.ptrs_trellis, C, ml.ptrs_suh, Ah, ml.ptrs_svh, idx,
-                       T(wts, cuda).view(1, 4), K, -1, ml.mcg, ml.mul1, -1, -1, 0)
-        ref = orc.exl3_mgemm(A[:1], trs, suhs, svhs, K, 2, npdt, indices=[3, 1, 0, 2], weights=wts, bszm_out=4)
-        assert rel_err(C[0].cpu().numpy(), ref[0])[0] <= tol
-        if golden is not None:
-            assert rel_err(C[0].cpu().numpy(), golden[f"mgemm_c_{int(fp32)}"])[0] <= 5e-3
-        # (d) expert-range filter [1, 3) with local tables
-        C = torch.zeros((4, m, n), dtype=dt, device=cuda)
-        ext.exl3_mgemm(T(A[:1], cuda), ml.ptrs_trellis[1:3].contiguous(), C, ml.ptrs_suh[1:3].contiguous(), Ah,
-                       ml.ptrs_svh[1:3].contiguous(), idx, T(wts, cuda).view(1, 4), K, -1, ml.mcg, ml.mul1, 1, 3, 0)
-        ref = orc.exl3_mgemm(A[:1], trs[1:3], suhs[1:3], svhs[1:3], K, 2, npdt, indices=[3, 1, 0, 2], weights=wts,
-                             min_index=1, max_index=3, bszm_out=4)
-        assert rel_err(C[0].cpu().numpy(), ref[0])[0] <= tol
-        if golden is not None:
-            assert rel_err(C[0].cpu().numpy(), golden[f"mgemm_d_{int(fp32)}"])[0] <= 5e-3
+    tags = set()
+
+    def model(tag, C, A_, npdt, what, slots=slice(None), **kw):
+        """C of a tag-100 / 200 call against oracle.exl3_mgemm_f16_model"""
+        tags.add(tag)
+        if tag in (ext.EXL3B_TAG_SIMT, ext.EXL3B_TAG_TC):
+            ref, tol = orc.exl3_mgemm_f16_model(A_, trs, suhs, svhs, K, 2, npdt, bszm_out=4, **kw)
+            check_f16_model(C.cpu().numpy()[slots], ref[slots], None if tol is None else tol[slots], what)
+
+    for path in (0, ext.EXL3B_TAG_SIMT):
+        prev = ext.set_gemm_path(path)
+        try:
+            for fp32 in (False, True):
+                dt = torch.float if fp32 else torch.half
+                npdt = np.float32 if fp32 else np.float16
+                Ah = torch.empty((4, m, k), dtype=torch.half, device=cuda)
+                tol = 3e-3
+                # (a) one input, four outputs
+                C = torch.zeros((4, m, n), dtype=dt, device=cuda)
+                tag = ext.exl3_mgemm(T(A[:1], cuda), ml.ptrs_trellis, C, ml.ptrs_suh, Ah, ml.ptrs_svh, None, None, K, -1,
+                                     ml.mcg, ml.mul1, -1, -1, 0)
+                ref = orc.exl3_mgemm(A[:1], trs, suhs, svhs, K, 2, npdt, bszm_out=4)
+                assert rel_err(C.cpu().numpy(), ref)[0] <= tol
+                model(tag, C, A[:1], npdt, (path, "a", fp32))
+                if golden is not None:
+                    assert rel_err(C.cpu().numpy(), golden[f"mgemm_a_{int(fp32)}"])[0] <= 5e-3
+                # (b) indices with a skipped slot
+                C = torch.zeros((4, m, n), dtype=dt, device=cuda)
+                idx = torch.tensor([[2, -1, 0, 3]], dtype=torch.long, device=cuda)
+                tag = ext.exl3_mgemm(T(A, cuda), ml.ptrs_trellis, C, ml.ptrs_suh, Ah, ml.ptrs_svh, idx, None, K, -1,
+                                     ml.mcg, ml.mul1, -1, -1, 0)
+                ref = orc.exl3_mgemm(A, trs, suhs, svhs, K, 2, npdt, indices=[2, -1, 0, 3], bszm_out=4)
+                assert rel_err(C.cpu().numpy(), ref)[0] <= tol and float(C[1].abs().max()) == 0.0
+                model(tag, C, A, npdt, (path, "b", fp32), indices=[2, -1, 0, 3])
+                if golden is not None:
+                    assert rel_err(C.cpu().numpy(), golden[f"mgemm_b_{int(fp32)}"])[0] <= 5e-3
+                # (c) weighted reduction into C[0]
+                C = torch.zeros((4, m, n), dtype=dt, device=cuda)
+                idx = torch.tensor([[3, 1, 0, 2]], dtype=torch.long, device=cuda)
+                tag = ext.exl3_mgemm(T(A[:1], cuda), ml.ptrs_trellis, C, ml.ptrs_suh, Ah, ml.ptrs_svh, idx,
+                                     T(wts, cuda).view(1, 4), K, -1, ml.mcg, ml.mul1, -1, -1, 0)
+                ref = orc.exl3_mgemm(A[:1], trs, suhs, svhs, K, 2, npdt, indices=[3, 1, 0, 2], weights=wts, bszm_out=4)
+                assert rel_err(C[0].cpu().numpy(), ref[0])[0] <= tol
+                model(tag, C, A[:1], npdt, (path, "c", fp32), slots=slice(0, 1), indices=[3, 1, 0, 2], weights=wts)
+                if golden is not None:
+                    assert rel_err(C[0].cpu().numpy(), golden[f"mgemm_c_{int(fp32)}"])[0] <= 5e-3
+                # (d) expert-range filter [1, 3) with local tables
+                C = torch.zeros((4, m, n), dtype=dt, device=cuda)
+                tag = ext.exl3_mgemm(T(A[:1], cuda), ml.ptrs_trellis[1:3].contiguous(), C, ml.ptrs_suh[1:3].contiguous(), Ah,
+                                     ml.ptrs_svh[1:3].contiguous(), idx, T(wts, cuda).view(1, 4), K, -1, ml.mcg, ml.mul1, 1, 3, 0)
+                ref = orc.exl3_mgemm(A[:1], trs[1:3], suhs[1:3], svhs[1:3], K, 2, npdt, indices=[3, 1, 0, 2], weights=wts,
+                                     min_index=1, max_index=3, bszm_out=4)
+                assert rel_err(C[0].cpu().numpy(), ref[0])[0] <= tol
+                if golden is not None:
+                    assert rel_err(C[0].cpu().numpy(), golden[f"mgemm_d_{int(fp32)}"])[0] <= 5e-3
+        finally:
+            ext.set_gemm_path(prev)
+    assert ext.EXL3B_TAG_SIMT in tags
 
 
 @pytest.mark.parametrize("K", [1, 2, 3, 4, 5, 6, 7, 8])

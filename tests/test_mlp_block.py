@@ -5,13 +5,15 @@ activation in its input stage (exl3_gemm_gated) and the blocks built on them (BC
 Bars: the operators are within 1 fp16 ulp of fp16(fp64 model) and exact where the model is (g = 0, relu2 at g <= 0);
 exl3_gemm_gated and the blocks are bit-identical to the reference's launch sequence composed from this library's operators
 (act_mul into a buffer, then exl3_gemm), on the same path; the gated block also meets the fp64-oracle bars of
-tests/test_gpu_parity.py.  Every exl3_gemm_gated output is written between sentinel rows that must keep their bits.
+tests/test_gpu_parity.py.  Every exl3_gemm_gated output is written between sentinel rows that must keep their bits; on tags 100 and
+200 it is also held to the exact model of the fp16 path on the activation's output (test_edges_host.check_f16_gemm).
 """
 import contextlib
 import numpy as np
 import pytest
 import torch
 from oracle import exl3_oracle as orc
+from test_edges_host import check_f16_gemm
 
 pytestmark = pytest.mark.gpu
 
@@ -168,6 +170,10 @@ def gated_vs_composed(dev, mt, m, act, limit, gu_dt, c_dt, force=0, seed=0):
     it = SENTINEL[c_dt][0]
     assert torch.equal(C1.view(it), C2.view(it)), ("not bit-identical", m, mt.k, mt.n, mt.K, mt.cb, act, limit, gu_dt, c_dt, force)
     assert torch.isfinite(C2).all()
+    if tag2 in (100, 200):
+        np_ = lambda t: t.cpu().numpy()
+        check_f16_gemm(np_(C2), np_(a), np_(mt.tr), np_(mt.suh), np_(mt.svh), mt.K, mt.cb, c_dt == torch.float,
+                       ("gated", m, mt.k, mt.n, mt.K, mt.cb, act, limit, force))
     return tag2
 
 

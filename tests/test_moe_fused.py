@@ -6,12 +6,14 @@ exl3_moe, the fused routed-expert MLP (csrc/moe_tc.cu, tag 230), against two ref
   * a composition of verified operators: per expert ext.exl3_gemm on the exact tensor-core path (tag 200) for gate and up,
     the activation in torch, ext.exl3_gemm for down, a weighted index_add.
 Bars (README "parity"): max-abs <= 4e-3 * max|y|, rel-RMS <= 2e-3.  Rows of tokens with no processed position keep their bits.
+Every case is also held to the exact model of the operator's arithmetic, oracle.exl3_moe_model (test_edges_host.check_moe_model).
 """
 import zlib
 import numpy as np
 import pytest
 import torch
 from oracle import exl3_oracle as orc
+from test_edges_host import check_moe_model
 
 pytestmark = pytest.mark.gpu
 
@@ -50,7 +52,7 @@ class Experts:
     def W(self, name, u):
         key = (name, u)
         if key not in self.w:
-            self.w[key] = orc.reconstruct(self.np[name][u][0], self.K[name], self.cb).astype(np.float64)
+            self.w[key] = orc.reconstruct(self.np[name][u][0], self.K[name], self.cb)
         return self.w[key]
 
     def gemm64(self, name, e, x):
@@ -192,6 +194,9 @@ def run_case(dev, E, topk, bsz, hidden, inter, Ks, cb, act, limit, T_, seed, sen
     assert np.isfinite(y[touched]).all()
     mx, rms = bars(y[touched], comp[touched])
     assert mx <= 4e-3 and rms <= 2e-3, f"vs composition: max {mx:.2e} rms {rms:.2e}"
+    mats = {name: [ex.np[name][e % ex.uniq] + (ex.K[name], ex.W(name, e % ex.uniq)) for e in range(E)] for name in ex.np}
+    model = orc.exl3_moe_model(x, out0, count, tok, wts, T_, act, limit, mats, cb)
+    check_moe_model(y[touched], model[touched], "vs exact model")
     if fp64:
         mx, rms = bars(y[touched], ref64[touched])
         assert mx <= 4e-3 and rms <= 2e-3, f"vs fp64 oracle: max {mx:.2e} rms {rms:.2e}"

@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 from oracle import exl3_oracle as orc
+from test_edges_host import check_f16_model
 
 
 
@@ -98,6 +99,8 @@ def test_routed_i8_mgemm_moe_modes(cuda, K, m):
             ext.set_gemm_path(ext.EXL3B_TAG_SIMT)
             Cs, tag_s, _ = run(xs, [6, 1, 3], wts)
             assert tag_s == ext.EXL3B_TAG_SIMT
+            model, mtol = orc.exl3_mgemm_f16_model(xs, trl, sul, svl, K, 2, npdt, indices=[6, 1, 3], weights=wts, bszm_out=topk)
+            check_f16_model(Cs[0].astype(npdt), model[0], None if mtol is None else mtol[0], ("simt", K, m, fp32))
             ext.set_gemm_path(ext.EXL3B_TAG_TC_I8_ROUTED)
             Ct, _, _ = run(xs, [6, 1, 3], wts)
             assert rel_err(Ct[0], Cs[0])[0] <= 2 * tol
@@ -162,9 +165,11 @@ def test_mgemm_split_matches_fused_default(cuda, monkeypatch, m, cb):
         outs[split] = C.cpu().numpy()
     for j in range(nm):
         ref = orc.exl3_gemm_f64(x[0], mats[j][0], mats[j][1], mats[j][2], K, cb)
+        model, _ = orc.exl3_gemm_f16_model(x[0], mats[j][0], mats[j][1], mats[j][2], K, cb, np.float32)
         for split in (False, True):
             mx, rms = rel_err(outs[split][j], ref)
             assert mx <= 2e-3 and rms <= 1e-3, (split, j, mx, rms)
+            check_f16_model(outs[split][j], model, None, (split, j))
 
 
 @pytest.mark.gpu

@@ -23,7 +23,7 @@ import numpy as np
 import pytest
 import torch
 from oracle import exl3_oracle as orc
-from test_edges_host import CACHE_PAIRS, gemm_plan
+from test_edges_host import CACHE_PAIRS, check_f16_model, gemm_plan
 
 gpu = pytest.mark.gpu
 
@@ -385,6 +385,15 @@ def test_skipped_slot_in_weighted_batch(cuda):
 
 # ---- 7. path selection and fallbacks ---------------------------------------------------------------------------------------
 
+def check_f16_slots(ex, c, y, what):
+    """A tag-100 call against the exact model of the fp16 paths (oracle.exl3_mgemm_f16_model), slot by slot."""
+    trl = [ex.tr[e % ex.uniq] for e in range(ex.E)]
+    ref, tol = orc.exl3_mgemm_f16_model(c.A, trl, ex.suh, ex.svh, ex.K, ex.cb, np.float32 if c.fp32 else np.float16, bszm_out=c.c_b,
+                                        **c.kw())
+    for j in range(c.c_b):
+        check_f16_model(y[j], ref[j], None if tol is None else tol[j], (what, j))
+
+
 @gpu
 def test_cuda_core_fallbacks(cuda):
     """m = 5, the mcg and 3inst codebooks and a forced EXL3B_TAG_SIMT go to tag 100: oracle bar and the reduce bit for bit."""
@@ -401,9 +410,11 @@ def test_cuda_core_fallbacks(cuda):
         try:
             for fp32 in (True, False):
                 what = (cb, m, force, fp32)
-                run(cuda, ex, x, idx, fp32=fp32, tag=TAG_SIMT, what=what, model=False)
+                c, y = run(cuda, ex, x, idx, fp32=fp32, tag=TAG_SIMT, what=what, model=False)
+                check_f16_slots(ex, c, y, what)
                 c, y = check_reduce(cuda, ex, A, idx, w, fp32, 2, tag=TAG_SIMT, what=what)
                 c.check(y, what, model=False)
+                check_f16_slots(ex, c, y, what)
         finally:
             ext.set_gemm_path(prev)
 
