@@ -138,6 +138,21 @@ static int check_kcb(int K, int cb)
     return 0;
 }
 
+// The size checks of the GEMM entries, after the entry's own argument checks: the entry's lower bounds (m >= m_min, k and
+// n >= kn_min, else the message `bounds`), then k and n multiples of 128 (messages prefixed with `who`).  Fills the shape
+// fields of *g; the caller sets the pointers.
+static int gemm_args(const char* who, const char* bounds, int m_min, int kn_min, int m, int k, int n, int K, int cb, int c_fp32,
+                     int force_num_sms, GemmArgs* g)
+{
+    EXL3B_CHECK(m >= m_min && k >= kn_min && n >= kn_min, EXL3B_ERR_SHAPE, "%s", bounds);
+    EXL3B_CHECK(k % 128 == 0, EXL3B_ERR_SHAPE, "%s: k (%d) must be divisible by 128", who, k);
+    EXL3B_CHECK(n % 128 == 0, EXL3B_ERR_SHAPE, "%s: n (%d) must be divisible by 128", who, n);
+    *g = GemmArgs{};
+    g->m = m; g->k = k; g->n = n; g->K = K; g->cb = cb; g->c_fp32 = c_fp32 != 0; g->out_scale = 1.0f;
+    g->max_ctas = force_num_sms > 0 ? force_num_sms : 0;
+    return 0;
+}
+
 int exl3b_had_r_128(void* stream, const void* in, void* out, const void* pre_scale, const void* post_scale,
                     float scale, int rows, int cols, int is_fp32)
 {
@@ -220,12 +235,9 @@ int exl3b_gemm_plan(int m, int k, int n, int K, int cb, int num_sms, int force_n
 {
     int r = check_kcb(K, cb); if (r) return r;
     EXL3B_CHECK(out, EXL3B_ERR_ARG, "exl3_gemm_plan: null output");
-    EXL3B_CHECK(m >= 1 && k >= 128 && n >= 128, EXL3B_ERR_SHAPE, "exl3_gemm_plan: empty problem");
-    EXL3B_CHECK(k % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm: k (%d) must be divisible by 128", k);
-    EXL3B_CHECK(n % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm: n (%d) must be divisible by 128", n);
+    GemmArgs g;
+    r = gemm_args("exl3_gemm", "exl3_gemm_plan: empty problem", 1, 128, m, k, n, K, cb, 0, force_num_sms, &g); if (r) return r;
     EXL3B_CHECK(num_sms >= 1, EXL3B_ERR_ARG, "exl3_gemm_plan: num_sms must be positive");
-    GemmArgs g{};
-    g.m = m; g.k = k; g.n = n; g.K = K; g.cb = cb; g.max_ctas = force_num_sms > 0 ? force_num_sms : 0;
     const int path = select_gemm_path(g);
     if (path < 0) return path;
     memset(out, 0, sizeof(*out));
@@ -238,7 +250,7 @@ int exl3b_gemm_plan(int m, int k, int n, int K, int cb, int num_sms, int force_n
     if (r) return r;
     out->passes = path == EXL3B_TAG_TC ? (m + 127) / 128 : 1;
     out->rows = pl.rows; out->grid = pl.grid; out->stages = pl.stages; out->smem_bytes = pl.smem_total;
-    out->a_stages = pl.a_stages; out->d_bufs = pl.d_bufs; out->tmem_cols = pl.tmem_cols; out->units = pl.units;
+    out->d_bufs = pl.d_bufs; out->units = pl.units;
     return 0;
 }
 
@@ -261,17 +273,12 @@ int exl3b_gemm(void* stream_, const void* A, const void* B, void* C, const void*
     cudaStream_t stream = (cudaStream_t) stream_;
     int r = check_kcb(K, cb); if (r) return r;
     EXL3B_CHECK(force_shape_idx <= 2, EXL3B_ERR_ARG, "exl3_gemm: force_shape_idx %d out of range (1 = CUDA-core, 2 = tensor-core)", force_shape_idx);
-    EXL3B_CHECK(m >= 0 && k >= 0 && n >= 0, EXL3B_ERR_SHAPE, "exl3_gemm: negative size");
-    EXL3B_CHECK(k % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm: k (%d) must be divisible by 128", k);
-    EXL3B_CHECK(n % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm: n (%d) must be divisible by 128", n);
+    GemmArgs g;
+    r = gemm_args("exl3_gemm", "exl3_gemm: negative size", 0, 0, m, k, n, K, cb, c_fp32, force_num_sms, &g); if (r) return r;
     if (m == 0 || n == 0) return EXL3B_TAG_NOP;
     EXL3B_CHECK(A && B && C, EXL3B_ERR_ARG, "exl3_gemm: null tensor");
     DevCtx* ctx; r = get_ctx(&ctx); if (r) return r;
-
-    GemmArgs g{};
     g.A = (const half*) A; g.suh = (const half*) suh; g.A_had = (half*) A_had; g.B = (const uint32_t*) B; g.C = C; g.svh = (const half*) svh;
-    g.m = m; g.k = k; g.n = n; g.K = K; g.cb = cb; g.c_fp32 = c_fp32 != 0; g.out_scale = 1.0f;
-    g.max_ctas = force_num_sms > 0 ? force_num_sms : 0;
 
     int path = select_gemm_path(g, force_shape_idx);
     if (path < 0) return path;
@@ -298,19 +305,15 @@ int exl3b_gemm_gated(void* stream, const void* G, const void* U, const void* B, 
 {
     int r = check_kcb(K, cb); if (r) return r;
     EXL3B_CHECK(act >= ACT_SILU && act <= ACT_RELU2, EXL3B_ERR_ARG, "exl3_gemm_gated: act must be 0 (SiLU), 1 (GELU) or 2 (ReLU^2), got %d", act);
-    EXL3B_CHECK(m >= 0 && k >= 0 && n >= 0, EXL3B_ERR_SHAPE, "exl3_gemm_gated: negative size");
-    EXL3B_CHECK(k % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm_gated: k (%d) must be divisible by 128", k);
-    EXL3B_CHECK(n % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm_gated: n (%d) must be divisible by 128", n);
+    GemmArgs g;
+    r = gemm_args("exl3_gemm_gated", "exl3_gemm_gated: negative size", 0, 0, m, k, n, K, cb, c_fp32, force_num_sms, &g); if (r) return r;
     if (m == 0 || n == 0) return EXL3B_TAG_NOP;
     EXL3B_CHECK(m <= 8, EXL3B_ERR_UNSUPPORTED, "exl3_gemm_gated: gated input is implemented for 1..8 rows, got %d", m);
     EXL3B_CHECK(G && U && B && C, EXL3B_ERR_ARG, "exl3_gemm_gated: null tensor");
     const uintptr_t align = gu_fp32 ? 16 : 8;
     EXL3B_CHECK((uintptr_t) G % align == 0 && (uintptr_t) U % align == 0, EXL3B_ERR_ARG,
                 "exl3_gemm_gated: G and U must be %d-byte aligned", (int) align);
-    GemmArgs g{};
-    g.A = nullptr; g.suh = (const half*) suh; g.A_had = nullptr; g.B = (const uint32_t*) B; g.C = C; g.svh = (const half*) svh;
-    g.m = m; g.k = k; g.n = n; g.K = K; g.cb = cb; g.c_fp32 = c_fp32 != 0; g.out_scale = 1.0f;
-    g.max_ctas = force_num_sms > 0 ? force_num_sms : 0;
+    g.suh = (const half*) suh; g.B = (const uint32_t*) B; g.C = C; g.svh = (const half*) svh;
     const int path = select_gemm_path(g);
     if (path < 0) return path;
     EXL3B_CHECK(path == EXL3B_TAG_TC || (path == EXL3B_TAG_TC_I8 && m <= 4), EXL3B_ERR_UNSUPPORTED,
@@ -326,14 +329,11 @@ int exl3b_gemm_allreduce(void* stream_, const void* A, const void* B, void* C, c
 {
     (void) A_had;                                   // the transform runs inside the kernel (m <= 4): no scratch is written
     int r = check_kcb(K, cb); if (r) return r;
-    EXL3B_CHECK(m >= 1 && k >= 0 && n >= 0, EXL3B_ERR_SHAPE, "exl3_gemm_allreduce: bad size");
-    EXL3B_CHECK(k % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm_allreduce: k (%d) must be divisible by 128", k);
-    EXL3B_CHECK(n % 128 == 0, EXL3B_ERR_SHAPE, "exl3_gemm_allreduce: n (%d) must be divisible by 128", n);
+    GemmArgs g;
+    r = gemm_args("exl3_gemm_allreduce", "exl3_gemm_allreduce: bad size", 1, 0, m, k, n, K, cb, c_fp32, 0, &g); if (r) return r;
     EXL3B_CHECK(A && B && C, EXL3B_ERR_ARG, "exl3_gemm_allreduce: null tensor");
     DevCtx* ctx; r = get_ctx(&ctx); if (r) return r;
-    GemmArgs g{};
-    g.A = (const half*) A; g.suh = (const half*) suh; g.A_had = nullptr; g.B = (const uint32_t*) B; g.C = C; g.svh = (const half*) svh;
-    g.m = m; g.k = k; g.n = n; g.K = K; g.cb = cb; g.c_fp32 = c_fp32 != 0; g.out_scale = 1.0f; g.max_ctas = 0;
+    g.A = (const half*) A; g.suh = (const half*) suh; g.B = (const uint32_t*) B; g.C = C; g.svh = (const half*) svh;
     return launch_gemm_tc_i8_ar((cudaStream_t) stream_, ctx, g);
 }
 

@@ -601,10 +601,8 @@ struct Chain
 
 const char* chain_op_unsupported(int m, int k, int n, int K, int cb, int in_mode)
 {
-    if (cb != 2) return "needs the mul1 codebook";
-    if (m < 1 || m > CH_MR) return "needs 1 <= m <= 4";
-    if (K < 1 || K > 8) return "K out of range";
-    if (k < 128 || n < 128 || k % 128 || n % 128) return "k and n must be multiples of 128";
+    static_assert(CH_MR == 4, "the chain takes the int8 rule's 1..4 rows");
+    if (const char* why = i8_shape_unsupported(m, k, n, K, cb, false)) return why;
     if (in_mode < 0 || in_mode > 2) return "in_mode must be 0 (fp16 rows), 1 (silu(gate) * up, fp32) or 2 (same, fp16)";
     if (in_mode != 0 && (size_t) m * k * 2 > I8_CACHE_MAX_BYTES) return "gated input needs m * k <= 32768";
     return nullptr;

@@ -114,7 +114,7 @@ struct TcPlan
     int smem_total;      // dynamic shared memory of the launch
     int grid;            // CTAs (single-matrix launch)
     long long units;     // 128 x 128 work units
-    int a_stages, d_bufs, tmem_cols;
+    int d_bufs;          // accumulator hand-off buffers
 };
 int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* pl);
 int plan_gemm_tc(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* pl);     // m <= 256: one pass
@@ -129,6 +129,10 @@ struct MGemmArgs;
 bool mgemm_tc_i8_supported(const DevCtx* ctx, const MGemmArgs& a);
 int launch_mgemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a);
 bool gemm_tc_i8_supported(const GemmArgs& a);
+// The int8 decode-GEMM's shape rule (gemm_tc_i8.cu), for every launch of its kernels: the mul1 codebook, 1..4 rows (5..8 too
+// when rows8 and the activation fits the shared-memory cache), K in 1..8, k and n multiples of 128.  nullptr = supported,
+// else the reason, which exl3b_gemm_allreduce_check and exl3_chain show to users.
+const char* i8_shape_unsupported(int m, int k, int n, int K, int cb, bool rows8);
 
 // tensor-parallel row-parallel GEMM with the sum over ranks fused into the epilogue (gemm_tc_i8_ar.cu)
 int launch_gemm_tc_i8_ar(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a);

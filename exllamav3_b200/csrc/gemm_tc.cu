@@ -371,9 +371,7 @@ int plan_gemm_tc(int m, int k, int n, int K, int num_sms, int max_ctas, TcPlan* 
 {
     EXL3B_CHECK(m >= 1 && m <= F16_MAX_ROWS, EXL3B_ERR_ARG, "plan_gemm_tc: one pass handles 1..%d rows", F16_MAX_ROWS);
     const int NT = (m + 15) / 16 * 16;
-    // accumulators live in the consumer warpgroups' registers: no operand stages or accumulator buffers to plan
-    pl->tmem_cols = 0;
-    pl->a_stages = 0;
+    // accumulators live in the consumer warpgroups' registers: no accumulator buffers to plan
     pl->d_bufs = 1;
     pl->b_load_bytes = m <= 8 ? 2048 : NT * 256;         // m <= 8: only the first row group is ever needed
     const int stages = f16_stages(K, NT);

@@ -1,5 +1,6 @@
-// Plain (single-GPU / column-parallel) instantiations and host side of the wgmma u8 x s8 EXL3 decode-GEMM;
-// the kernel itself is in gemm_tc_i8_body.cuh.
+// The kernel entries and the shared host side of the wgmma u8 x s8 EXL3 decode-GEMM: shape rule, launch geometry, launch
+// parameters and the launch itself, for the plain and gated (tag 210), row-parallel (tag 211, gemm_tc_i8_ar.cu) and routed
+// (tag 212, gemm_tc_i8_routed.cu) calls.  The kernel body is in gemm_tc_i8_body.cuh.
 #include "gemm_tc_i8_body.cuh"
 
 namespace exl3b {
@@ -22,24 +23,84 @@ gemm_tc_i8_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w, 
 template <int K, int MR> constexpr void (*i8_plain_kernel)(const TcParams, const CUtensorMap) = gemm_tc_i8_kernel<K, MR>;
 template <int K> constexpr void (*i8_gated_kernel)(const TcParams, const CUtensorMap, const GateIn) = gemm_tc_i8_kernel<K, 4>;
 
+// row-parallel: the epilogue sums the ranks' partial outputs over NVLink peer memory (gemm_tc_i8_ar.cu)
+template <int K>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_i8_ar_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ ArArgs ar)
+{
+    gemm_tc_i8_body<K, 4, true>(p, &tmap_w, &ar);
+}
+
+// routed: one CTA group per active slot of the call (gemm_tc_i8_routed.cu)
+template <int K>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_i8_routed_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ RouteArgs route)
+{
+    gemm_tc_i8_body<K, 4, false, true>(p, &tmap_w, nullptr, &route);
+}
+
 // ---- host side -------------------------------------------------------------------------------------------------------
 
+// the kernel entry of a launch: row-parallel (ar), routed (route), gated rows (gate) or plain rows
 template <int K>
-static cudaError_t i8_launch(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap,
-                             const GateIn* gate = nullptr)
+static cudaError_t i8_kernel(cudaStream_t stream, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap,
+                             const GateIn* gate, const ArArgs* ar, const RouteArgs* route)
 {
-    if (gate) return launch_pdl<i8_gated_kernel<K>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap, *gate);
-    return p.m <= 4 ? launch_pdl<i8_plain_kernel<K, 4>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap)
-                    : launch_pdl<i8_plain_kernel<K, 8>>(stream, dim3(grid), TC_THREADS, smem_bytes, p, tmap);
+    const dim3 g(grid);
+    if (ar) return launch_pdl<gemm_tc_i8_ar_kernel<K>>(stream, g, TC_THREADS, smem_bytes, p, tmap, *ar);
+    if (route) return launch_pdl<gemm_tc_i8_routed_kernel<K>>(stream, g, TC_THREADS, smem_bytes, p, tmap, *route);
+    if (gate) return launch_pdl<i8_gated_kernel<K>>(stream, g, TC_THREADS, smem_bytes, p, tmap, *gate);
+    return p.m <= 4 ? launch_pdl<i8_plain_kernel<K, 4>>(stream, g, TC_THREADS, smem_bytes, p, tmap)
+                    : launch_pdl<i8_plain_kernel<K, 8>>(stream, g, TC_THREADS, smem_bytes, p, tmap);
 }
 
-// rows 5..8 need the whole transformed activation cached in shared memory (the per-unit digit warps cannot afford eight Hadamards)
-static bool i8_rows_ok(int m, int k) { return m >= 1 && (m <= 4 || (m <= I8_MAX_M && (size_t) m * k * 2 <= I8_CACHE_MAX_BYTES)); }
-
-bool gemm_tc_i8_supported(const GemmArgs& a)
+int i8_launch(cudaStream_t stream, int K, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap, const GateIn* gate,
+              const ArArgs* ar, const RouteArgs* route)
 {
-    return a.cb == 2 && i8_rows_ok(a.m, a.k) && a.k >= 128 && a.n >= 128 && a.k % 128 == 0 && a.n % 128 == 0;
+    cudaError_t err = cudaSuccess;
+    EXL3B_DISPATCH_K(K, err = i8_kernel<KK>(stream, grid, smem_bytes, p, tmap, gate, ar, route));
+    count_launch();
+    EXL3B_CUDA(err);
+    EXL3B_CUDA(cudaPeekAtLastError());
+    return 0;
 }
+
+TcParams i8_params(DevCtx* ctx, int slot, const TcPlan& pl, const GemmArgs& a)
+{
+    TcParams p{};
+    p.A_raw = a.A; p.suh = a.suh; p.B = a.B; p.svh = a.svh; p.C = a.C;
+    p.m = a.m; p.k = a.k; p.n = a.n; p.NT = I8_NT; p.c_fp32 = a.c_fp32; p.out_scale = a.out_scale;
+    p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot); p.parts = ctx->i8_parts_slot(slot); p.dbg = g_tc_dbg;
+    p.stages = pl.stages; p.b_bytes = pl.b_bytes; p.b_load_bytes = pl.b_load_bytes;
+    return p;
+}
+
+TcParams i8_params(DevCtx* ctx, int slot, const TcPlan& pl, const MGemmArgs& a, int mats)
+{
+    GemmArgs g{};
+    g.A = a.A; g.C = a.C; g.m = a.m; g.k = a.k; g.n = a.n; g.c_fp32 = a.c_fp32; g.out_scale = 1.f;
+    TcParams p = i8_params(ctx, slot, pl, g);
+    p.num_mats = mats;                           // > 0 selects the table-driven path in the kernel
+    p.B_ptrs = a.B_ptrs; p.suh_ptrs = a.suh_ptrs; p.svh_ptrs = a.svh_ptrs;
+    p.a_mat_stride = a.bszm_in == 1 ? 0 : (long long) a.m * a.k;
+    p.c_mat_stride = (long long) a.m * a.n * (a.c_fp32 ? 4 : 2);
+    p.tmap_slots = ctx->tmap_slot(slot);
+    return p;
+}
+
+const char* i8_shape_unsupported(int m, int k, int n, int K, int cb, bool rows8)
+{
+    // rows 5..8 need the whole transformed activation cached in shared memory (the per-unit digit warps cannot afford eight
+    // Hadamards)
+    const bool rows_ok = m >= 1 && (m <= 4 || (rows8 && m <= I8_MAX_M && (size_t) m * k * 2 <= I8_CACHE_MAX_BYTES));
+    if (cb != 2) return "needs the mul1 codebook";
+    if (!rows_ok) return rows8 ? "needs 1 <= m <= 4, or m <= 8 with m * k <= 32768" : "needs 1 <= m <= 4";
+    if (K < 1 || K > 8) return "K out of range";
+    if (k < 128 || n < 128 || k % 128 || n % 128) return "k and n must be multiples of 128";
+    return nullptr;
+}
+
+bool gemm_tc_i8_supported(const GemmArgs& a) { return !i8_shape_unsupported(a.m, a.k, a.n, a.K, a.cb, true); }
 
 // rows variant, ring depth, activation cache and shared memory of a launch (single- and multi-matrix alike)
 static int plan_i8_smem(int m, int k, int K, TcPlan* pl)
@@ -69,7 +130,7 @@ int plan_gemm_tc_i8(int m, int k, int n, int K, int num_sms, int max_ctas, TcPla
     EXL3B_CHECK(n / 128 <= DevCtx::COUNTERS_PER_SLOT, EXL3B_ERR_UNSUPPORTED, "exl3_gemm: too many column strips");
     EXL3B_CHECK(grid <= DevCtx::I8_PART_CTAS, EXL3B_ERR_UNSUPPORTED, "exl3_gemm (i8): grid exceeds the split-K exchange buffer");
     EXL3B_CHECK(partition_fits(U, grid), EXL3B_ERR_UNSUPPORTED, "exl3_gemm (i8): too many units for the 32-bit stream-K partition");
-    pl->grid = grid; pl->units = U; pl->a_stages = 0; pl->d_bufs = 2; pl->tmem_cols = 0;
+    pl->grid = grid; pl->units = U; pl->d_bufs = 2;
     return 0;
 }
 
@@ -80,19 +141,8 @@ int launch_gemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a, const
     { int r = get_weight_tmap(a.B, a.k, a.n, a.K, &tmap); if (r) return r; }
     TcPlan pl;
     { int r = plan_gemm_tc_i8(a.m, a.k, a.n, a.K, ctx->num_sms, a.max_ctas, &pl); if (r) return r; }
-    const int slot = ctx->next_slot();
-    TcParams p{};
-    p.B = a.B; p.C = a.C; p.svh = a.svh; p.m = a.m; p.k = a.k; p.n = a.n; p.NT = I8_NT; p.c_fp32 = a.c_fp32;
-    p.out_scale = a.out_scale; p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot);
-    p.A_raw = a.A; p.suh = a.suh; p.dbg = g_tc_dbg;
-    p.parts = ctx->i8_parts_slot(slot);
-    p.stages = pl.stages; p.b_bytes = pl.b_bytes; p.b_load_bytes = pl.b_load_bytes;
-    const int grid = pl.grid, smem_total = pl.smem_total;
-    cudaError_t err = cudaSuccess;
-    EXL3B_DISPATCH_K(a.K, err = i8_launch<KK>(stream, grid, smem_total, p, tmap, gate));
-    count_launch();
-    EXL3B_CUDA(err);
-    EXL3B_CUDA(cudaPeekAtLastError());
+    const TcParams p = i8_params(ctx, ctx->next_slot(), pl, a);
+    { int r = i8_launch(stream, a.K, pl.grid, pl.smem_total, p, tmap, gate); if (r) return r; }
     return EXL3B_TAG_TC_I8;
 }
 
@@ -126,19 +176,18 @@ int plan_fanout_groups(int k, const int32_t* widths, int mats, int num_sms, int*
 bool mgemm_tc_i8_supported(const DevCtx* ctx, const MGemmArgs& a)
 {
     // dense case only: one output per matrix, shared or per-matrix input, no routing / weighting; per-matrix widths (fan-out) only
-    // when the caller registered a host copy of the width list (the launch geometry depends on it)
-    if (a.cb != 2 || !i8_rows_ok(a.m, a.k)) return false;
+    // when the caller registered a host copy of the width list (the launch geometry depends on it, and checks the widths)
+    if (i8_shape_unsupported(a.m, a.k, a.size_n_list ? 128 : a.n, a.K, a.cb, true)) return false;
     if (a.indices || a.weights || a.min_index >= 0 || a.num_tokens != 1) return false;
     if (a.size_n_list)
     {
-        if (!a.size_n_host || !a.c_ptrs || a.k < 128 || a.k % 128) return false;
+        if (!a.size_n_host || !a.c_ptrs) return false;
         if (!(a.bszm_in == 1 || a.bszm_in == a.bszm_out)) return false;
         int cta0[TC_RAG_MAX_MATS + 1];
         return plan_fanout_groups(a.k, a.size_n_host, a.bszm_out, ctx->num_sms, cta0) > 0;
     }
     if (a.bszm_out < 1 || !(a.bszm_in == 1 || a.bszm_in == a.bszm_out)) return false;
     if (a.bszm_out > ctx->num_sms || a.bszm_out > DevCtx::TMAP_SLOTS) return false;
-    if (a.k < 128 || a.n < 128 || a.k % 128 || a.n % 128) return false;
     if ((long long) a.bszm_out * (a.n / 128) > DevCtx::COUNTERS_PER_SLOT) return false;
     return true;
 }
@@ -152,19 +201,9 @@ int launch_mgemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a)
     CUtensorMap tmap;
     { int r = get_weight_tmap(ctx->ws, a.k, a.size_n_list ? 128 : a.n, a.K, &tmap); if (r) return r; }     // template: address patched per CTA (unused by fan-out launches)
     const int slot = ctx->next_slot();
-    TcParams p{};
-    p.C = a.C; p.m = a.m; p.k = a.k; p.n = a.n; p.NT = I8_NT; p.c_fp32 = a.c_fp32;
-    p.out_scale = 1.f; p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot);
-    p.A_raw = a.A; p.dbg = g_tc_dbg;
-    p.num_mats = mats;                           // > 0 selects the table-driven path in the kernel
-    p.B_ptrs = a.B_ptrs; p.suh_ptrs = a.suh_ptrs; p.svh_ptrs = a.svh_ptrs;
-    p.a_mat_stride = a.bszm_in == 1 ? 0 : (long long) a.m * a.k;
-    p.c_mat_stride = (long long) a.m * a.n * (a.c_fp32 ? 4 : 2);
-    p.tmap_slots = ctx->tmap_slot(slot);
-    p.parts = ctx->i8_parts_slot(slot);
     TcPlan pl;
     { int r = plan_i8_smem(a.m, a.k, a.K, &pl); if (r) return r; }
-    p.stages = pl.stages; p.b_bytes = pl.b_bytes; p.b_load_bytes = pl.b_load_bytes;
+    TcParams p = i8_params(ctx, slot, pl, a, mats);
     const long long U = (long long) (a.k / 128) * (a.n / 128);
     int gpm = ctx->num_sms / mats;
     if (gpm > U) gpm = (int) U;
@@ -179,11 +218,7 @@ int launch_mgemm_tc_i8(cudaStream_t stream, DevCtx* ctx, const MGemmArgs& a)
         EXL3B_CHECK(grid > 0, EXL3B_ERR_UNSUPPORTED, "exl3_mgemm (i8): fan-out widths not supported");
         for (int j = 0; j < mats; ++j) p.rag_n[j] = a.size_n_host[j];
     }
-    cudaError_t err = cudaSuccess;
-    EXL3B_DISPATCH_K(a.K, err = i8_launch<KK>(stream, grid, pl.smem_total, p, tmap));
-    count_launch();
-    EXL3B_CUDA(err);
-    EXL3B_CUDA(cudaPeekAtLastError());
+    { int r = i8_launch(stream, a.K, grid, pl.smem_total, p, tmap); if (r) return r; }
     return EXL3B_TAG_TC_I8;
 }
 

@@ -4,7 +4,7 @@
 //
 // Replaces, for the row-parallel linears of the reference's TP mode, the pair  exl3_gemm  +  all_reduce  that its callers
 // issue (modules/mlp.py:769-770, modules/attn.py:546-547 -> model/model_tp_backend.py:119-126, one NCCL launch per
-// output): the kernel is gemm_tc_i8_body<K, 4, AR = true> -- the same decode-GEMM, whose epilogue exchanges each finished
+// output): the kernel is gemm_tc_i8_body<K, 4, AR = true> (entry in gemm_tc_i8.cu) -- the same decode-GEMM, whose epilogue exchanges each finished
 // 128-column segment with the peer GPUs through NVLink peer memory (flag-in-data, see emit_rows in gemm_tc_i8_body.cuh).
 //
 // Setup (one process per GPU): every rank allocates a receive buffer (tp_alloc), the ranks exchange the 64-byte CUDA IPC
@@ -13,17 +13,10 @@
 //
 // STATUS: world-1 equality with the plain kernel and the loop-back protocol (scatter, rank-ordered sum, re-arming, slot
 // alternation) tested on one GPU; multi-GPU runs: tests/test_tp_fused.py -m multigpu, bench.py --gpus N.
-#include "gemm_tc_i8_body.cuh"
+#include "i8_pipeline.cuh"
 #include <mutex>
 
 namespace exl3b {
-
-template <int K>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-gemm_tc_i8_ar_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ ArArgs ar)
-{
-    gemm_tc_i8_body<K, 4, true>(p, &tmap_w, &ar);
-}
 
 // bring-up: place a "peer" partial into the own receive buffer, in the slot the NEXT row-parallel launch will read
 __global__ void tp_inject_kernel(const unsigned int* state, uint32_t* local, long long slot_elems, int world, int src,
@@ -198,10 +191,7 @@ long long tp_debug_epoch()
 // why a call cannot take the fused path (nullptr = it can); checked without touching the device
 const char* gemm_tc_i8_ar_unsupported(int m, int k, int n, int K, int cb, int world, long long slot_elems)
 {
-    if (cb != 2) return "needs the mul1 codebook";
-    if (m < 1 || m > 4) return "needs 1 <= m <= 4";
-    if (K < 1 || K > 8) return "K out of range";
-    if (k < 128 || n < 128 || k % 128 || n % 128) return "k and n must be multiples of 128";
+    if (const char* why = i8_shape_unsupported(m, k, n, K, cb, false)) return why;
     if (world < 1 || world > AR_MAX_WORLD) return "world size out of range";
     if ((long long) m * n > slot_elems) return "m * n exceeds the exchange slot (tp_alloc max_elems)";
     return nullptr;
@@ -218,23 +208,12 @@ int launch_gemm_tc_i8_ar(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
     CUtensorMap tmap;
     { int r = get_weight_tmap(a.B, a.k, a.n, a.K, &tmap); if (r) return r; }
     const int slot = ctx->next_slot();
-    TcParams p{};
-    p.B = a.B; p.C = a.C; p.svh = a.svh; p.m = a.m; p.k = a.k; p.n = a.n; p.NT = I8_NT; p.c_fp32 = a.c_fp32;
-    p.out_scale = a.out_scale; p.ws = ctx->ws_slot(slot); p.counters = ctx->counter_slot(slot);
-    p.A_raw = a.A; p.suh = a.suh; p.dbg = g_tc_dbg;
-    p.parts = ctx->i8_parts_slot(slot);
     TcPlan pl;
     { int r = plan_gemm_tc_i8(a.m, a.k, a.n, a.K, ctx->num_sms, a.max_ctas, &pl); if (r) return r; }      // m <= 4: the MR = 4 variant
-    p.stages = pl.stages; p.b_bytes = pl.b_bytes; p.b_load_bytes = pl.b_load_bytes;
-    const int grid = pl.grid;
     ArArgs ar{};
     for (int j = 0; j < g->world; ++j) ar.recv[j] = g->recv[j];
     ar.state = g->state; ar.slot_elems = g->slot_elems; ar.rank = g->rank; ar.world = g->world;
-    cudaError_t err = cudaSuccess;
-    EXL3B_DISPATCH_K(a.K, err = launch_pdl<gemm_tc_i8_ar_kernel<KK>>(stream, dim3(grid), TC_THREADS, pl.smem_total, p, tmap, ar));
-    count_launch();
-    EXL3B_CUDA(err);
-    EXL3B_CUDA(cudaPeekAtLastError());
+    { int r = i8_launch(stream, a.K, pl.grid, pl.smem_total, i8_params(ctx, slot, pl, a), tmap, nullptr, &ar); if (r) return r; }
     return EXL3B_TAG_TC_I8_AR;
 }
 

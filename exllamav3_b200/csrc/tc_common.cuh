@@ -141,4 +141,14 @@ __device__ __forceinline__ uint2 xt_transform(uint2 raw, const half* suh, int la
 int get_weight_tmap(const void* B, int k, int n, int K, CUtensorMap* out);
 extern unsigned long long* g_tc_dbg;
 
+// ---- int8 decode-GEMM launches (gemm_tc_i8.cu) ----------------------------------------------------------------------
+// The TcParams every int8 launch shares, on launch slot `slot` with plan `pl`: one matrix (a), or the pointer tables of `mats`
+// matrices (multi-matrix launches; g_per_mat and the fan-out fields are the caller's).
+TcParams i8_params(DevCtx* ctx, int slot, const TcPlan& pl, const GemmArgs& a);
+TcParams i8_params(DevCtx* ctx, int slot, const TcPlan& pl, const MGemmArgs& a, int mats);
+// One launch of the kernel entry the extra arguments select: plain rows, or gated rows (gate), the row-parallel sum (ar) or
+// routed slots (route).  Counted; 0 or the launch error.
+int i8_launch(cudaStream_t stream, int K, int grid, int smem_bytes, const TcParams& p, const CUtensorMap& tmap,
+              const GateIn* gate = nullptr, const ArArgs* ar = nullptr, const RouteArgs* route = nullptr);
+
 }  // namespace exl3b

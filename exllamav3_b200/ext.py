@@ -153,6 +153,34 @@ def _dtype(t, dt, name):
         raise RuntimeError(f"{name} is incorrect datatype, must be {dt}")
 
 
+def _contiguous(op: str, *ts):
+    for t in ts:
+        if t is not None and not t.is_contiguous():
+            raise RuntimeError(f"{op}: tensors must be contiguous")
+
+
+def _gemm_operands(op: str, A, B, C, *more, c_numel=False, a_name="A"):
+    """
+    Checks of a GEMM entry's (input A, trellis B, output C); the input's dtype is the caller's to check.  `more`: further inputs
+    that must be contiguous.  c_numel: C must also hold exactly m * n elements, not only n columns.  Returns (m, k, n, K, c_fp32).
+    """
+    if B.dim() != 3:
+        raise RuntimeError("B: incorrect number of dimensions, must be 3")
+    _dtype(B, torch.int16, "B")
+    c_fp32 = C.dtype == torch.float
+    if not c_fp32:
+        _dtype(C, torch.half, "C")
+    k = A.shape[-1]
+    m = A.numel() // k if k else 0
+    n, K = B.shape[1] * 16, B.shape[2] // 16
+    if k != B.shape[0] * 16:
+        raise RuntimeError(f"{a_name} and B incompatible shapes")
+    if C.shape[-1] != n or (c_numel and C.numel() != m * n):
+        raise RuntimeError("C and B incompatible shapes")
+    _contiguous(op, A, B, C, *more)
+    return m, k, n, K, c_fp32
+
+
 def launch_count() -> int:
     return int(_lib.exl3b_launch_count())
 
@@ -174,26 +202,12 @@ _forced_path = 0
 def exl3_gemm(A, B, C, suh, A_had, svh, force_shape_idx: int, mcg, mul1, force_num_sms: int) -> int:
     """A @ B -> C with EXL3-quantized B.  exllamav3_ext/quant/exl3_gemm.cu:110-339."""
     _need_cuda(A, B, C, suh, A_had, svh)
-    if B.dim() != 3:
-        raise RuntimeError("B: incorrect number of dimensions, must be 3")
     _dtype(A, torch.half, "A")
-    _dtype(B, torch.int16, "B")
-    c_fp32 = C.dtype == torch.float
-    if not c_fp32:
-        _dtype(C, torch.half, "C")
-    size_k = A.shape[-1]
-    size_m = A.numel() // size_k if size_k else 0
-    size_n = B.shape[1] * 16
-    if size_k != B.shape[0] * 16:
-        raise RuntimeError("A and B incompatible shapes")
-    if C.shape[-1] != size_n:
-        raise RuntimeError("C and B incompatible shapes")
-    K = B.shape[2] // 16
-    assert A.is_contiguous() and B.is_contiguous() and C.is_contiguous()
+    m, k, n, K, c_fp32 = _gemm_operands("exl3_gemm", A, B, C)
     with torch.cuda.device(A.device):
         return _check(_lib.exl3b_gemm(
             _stream(A), _ptr(A), _ptr(B), _ptr(C), _ptr(suh), _ptr(A_had) if suh is not None else None, _ptr(svh),
-            size_m, size_k, size_n, K, _cb(mcg, mul1), int(c_fp32), int(force_shape_idx), int(force_num_sms)))
+            m, k, n, K, _cb(mcg, mul1), int(c_fp32), int(force_shape_idx), int(force_num_sms)))
 
 
 # ---- GEMM chains: the quantized linears of a decode block as ONE persistent launch (include/exl3b200.h) --------------------
@@ -223,9 +237,6 @@ class GemmChain:
             x = o["gate"] if gated else o["x"]
             x2 = o["up"] if gated else None
             _need_cuda(x, x2, tr, y, o.get("suh"), o.get("svh"))
-            if tr.dim() != 3:
-                raise RuntimeError("B: incorrect number of dimensions, must be 3")
-            _dtype(tr, torch.int16, "B")
             if gated:
                 if x.dtype not in (torch.float, torch.half) or x2.dtype != x.dtype or x2.shape != x.shape:
                     raise RuntimeError("gate / up must be fp32 or fp16 tensors of one shape")
@@ -233,17 +244,7 @@ class GemmChain:
             else:
                 _dtype(x, torch.half, "A")
                 in_mode = 0
-            c_fp32 = y.dtype == torch.float
-            if not c_fp32:
-                _dtype(y, torch.half, "C")
-            k = x.shape[-1]
-            m = x.numel() // k if k else 0
-            n, K = tr.shape[1] * 16, tr.shape[2] // 16
-            if k != tr.shape[0] * 16:
-                raise RuntimeError("A and B incompatible shapes")
-            if y.shape[-1] != n or y.numel() != m * n:
-                raise RuntimeError("C and B incompatible shapes")
-            assert x.is_contiguous() and tr.is_contiguous() and y.is_contiguous() and (x2 is None or x2.is_contiguous())
+            m, k, n, K, c_fp32 = _gemm_operands("GemmChain", x, tr, y, x2, c_numel=True)
             if dev is None:
                 dev = tr.device
             elif tr.device != dev:
@@ -318,54 +319,69 @@ def exl3_gemm_allreduce(A, B, C, suh, A_had, svh, mcg, mul1) -> int:
     eligible (mul1, rows <= 4, group attached, rows * n within the exchange slot); the caller then uses exl3_gemm + NCCL.
     """
     _need_cuda(A, B, C, suh, A_had, svh)
-    if B.dim() != 3:
-        raise RuntimeError("B: incorrect number of dimensions, must be 3")
     _dtype(A, torch.half, "A")
-    _dtype(B, torch.int16, "B")
-    c_fp32 = C.dtype == torch.float
-    if not c_fp32:
-        _dtype(C, torch.half, "C")
-    size_k = A.shape[-1]
-    size_m = A.numel() // size_k if size_k else 0
-    size_n = B.shape[1] * 16
-    if size_k != B.shape[0] * 16:
-        raise RuntimeError("A and B incompatible shapes")
-    if C.shape[-1] != size_n:
-        raise RuntimeError("C and B incompatible shapes")
-    K = B.shape[2] // 16
-    assert A.is_contiguous() and B.is_contiguous() and C.is_contiguous()
+    m, k, n, K, c_fp32 = _gemm_operands("exl3_gemm_allreduce", A, B, C)
     with torch.cuda.device(A.device):
         return _check(_lib.exl3b_gemm_allreduce(
-            _stream(A), _ptr(A), _ptr(B), _ptr(C), _ptr(suh), None, _ptr(svh),
-            size_m, size_k, size_n, K, _cb(mcg, mul1), int(c_fp32)))
+            _stream(A), _ptr(A), _ptr(B), _ptr(C), _ptr(suh), None, _ptr(svh), m, k, n, K, _cb(mcg, mul1), int(c_fp32)))
 
 
 # Dense exl3_mgemm calls the int8 tensor-core kernel cannot take (other codebooks, or 5..32 rows: the reference's model code
 # fuses k+v and gate+up up to 32 rows, modules/attn.py:603, modules/mlp.py:726) are issued as one exact tensor-core exl3_gemm per
 # matrix (tag 200; same results as separate calls, checked against the fused CUDA-core kernels by the tests).  That needs the
-# pointer tables' VALUES on the host, so each table tensor is copied back once and remembered for as long as that tensor
-# object lives and is not modified (weak reference + version counter; never keyed on an address, which the caching allocator
-# reuses).  A table first seen during CUDA-graph capture cannot be copied: such a call runs on the CUDA-core multi-matrix
-# kernels (tag 100), as does everything with EXL3B_MGEMM_SPLIT=0.
+# pointer tables' VALUES on the host, so each table tensor is copied back once (_host_copy, keyed on the tensor object).  A
+# table first seen during CUDA-graph capture cannot be copied: such a call runs on the CUDA-core multi-matrix kernels
+# (tag 100), as does everything with EXL3B_MGEMM_SPLIT=0.
 _MGEMM_SPLIT = os.environ.get("EXL3B_MGEMM_SPLIT", "1") != "0"
-_table_cache: dict = {}
 
 
-def _host_table(t: torch.Tensor):
-    key = id(t)
-    ent = _table_cache.get(key)
-    if ent is not None and ent[0]() is t and ent[1] == t._version:
-        return ent[2]
-    if t.is_cuda and torch.cuda.is_current_stream_capturing():
+def _capturing() -> bool:
+    """Whether the current CUDA stream is capturing a graph; a process without a usable CUDA driver captures nothing."""
+    try:
+        return torch.cuda.is_current_stream_capturing()
+    except RuntimeError:
+        return False
+
+
+def _host_copy(cache: dict, key, t: torch.Tensor, mirror=None):
+    """
+    The values of integer tensor `t` as a host list, copied once and kept in `cache` under `key` for as long as that tensor object
+    lives and is not modified.  An entry is trusted only for the very object it was made from (a freed tensor's address is reused
+    by the caching allocator, found the hard way) at the same version (in-place writes bump it).  The copy synchronises, so
+    during stream capture nothing is copied and None is returned.  mirror(key, values) is told of each new copy, and
+    mirror(key, None) when the entry is withdrawn: the object died, or another object or version replaced it.
+    """
+    hit = cache.get(key)
+    if hit is not None:
+        if hit[0]() is t and hit[1] == t._version:
+            return hit[2]
+        _forget_copy(cache, key, hit[0])
+    if _capturing():
         return None
     vals = [int(v) for v in t.detach().cpu().tolist()]
-    _table_cache[key] = (weakref.ref(t, lambda _r, key=key: _table_cache.pop(key, None)), t._version, vals)
+    if mirror is not None:
+        mirror(key, vals)
+    cache[key] = (weakref.ref(t, lambda r, key=key, forget=_forget_copy: forget(cache, key, r)), t._version, vals, mirror)
     return vals
+
+
+def _forget_copy(cache: dict, key, ref) -> None:
+    hit = cache.get(key)
+    if hit is not None and hit[0] is ref:
+        del cache[key]
+        if hit[3] is not None:
+            try:
+                hit[3](key, None)
+            except Exception:                      # interpreter shutdown
+                pass
+
+
+_table_cache: dict = {}                            # id(table tensor) -> host copy
 
 
 def _mgemm_split(A, B, C, suh, A_had, svh, K, cb, c_fp32, bszm_in, bszm_out, m, k, n, force_num_sms):
     """One exl3b_gemm per matrix for a dense multi-matrix call; returns the path tag or None if the tables are unavailable."""
-    tb, ts, tv = _host_table(B), _host_table(suh), _host_table(svh)
+    tb, ts, tv = (_host_copy(_table_cache, id(t), t) for t in (B, suh, svh))
     if tb is None or ts is None or tv is None or len(tb) < bszm_out:
         return None
     a0, c0, h0 = A.data_ptr(), C.data_ptr(), A_had.data_ptr()
@@ -380,41 +396,18 @@ def _mgemm_split(A, B, C, suh, A_had, svh, K, cb, c_fp32, bszm_in, bszm_out, m, 
     return tag
 
 
-# size_n_list tensors whose host copy the library knows: device address -> (weak reference to THE tensor object, torch version
-# counter, widths).  An entry is trusted only for the very tensor object it was made from (a freed tensor's address is reused by
-# the caching allocator, found the hard way) at the same version (in-place writes bump it); when that object dies the entry is
-# withdrawn from the library.  The copy to the host synchronises, so it happens on the first call with a tensor object -- never
-# during stream capture: an unknown list simply takes the generic path there.
+# size_n_list tensors whose host copy the library knows (exl3b_register_widths, keyed by device address), mirrored by a host copy
+# here.  An unknown list (first seen during stream capture) simply takes the generic path.
 _widths_known: dict = {}
 
 
-def _forget_widths(key: int, ref) -> None:
-    hit = _widths_known.get(key)
-    if hit is not None and hit[0] is ref:
-        del _widths_known[key]
-        try:
-            _lib.exl3b_register_widths(ctypes.c_void_p(key), None, 0)
-        except Exception:                          # interpreter shutdown
-            pass
+def _library_widths(key: int, widths) -> None:
+    n = 0 if widths is None else len(widths)
+    _check(_lib.exl3b_register_widths(ctypes.c_void_p(key), (ctypes.c_int32 * n)(*widths) if n else None, n))
 
 
 def _register_widths(size_n_list) -> None:
-    import weakref
-    key = size_n_list.data_ptr()
-    ver = size_n_list._version
-    hit = _widths_known.get(key)
-    if hit is not None and hit[0]() is size_n_list and hit[1] == ver:
-        return
-    if hit is not None:                            # another tensor at this address, or rewritten: the library must not trust it
-        del _widths_known[key]
-        _lib.exl3b_register_widths(ctypes.c_void_p(key), None, 0)
-    if torch.cuda.is_current_stream_capturing():
-        return
-    widths = [int(v) for v in size_n_list.detach().cpu().tolist()]
-    arr = (ctypes.c_int32 * len(widths))(*widths)
-    _check(_lib.exl3b_register_widths(ctypes.c_void_p(key), arr, len(widths)))
-    ref = weakref.ref(size_n_list, lambda r, key=key: _forget_widths(key, r))
-    _widths_known[key] = (ref, ver, widths)
+    _host_copy(_widths_known, size_n_list.data_ptr(), size_n_list, _library_widths)
 
 
 def plan_fanout(k: int, widths, num_sms: int):
@@ -474,7 +467,7 @@ def exl3_mgemm(A, B, C, suh, A_had, svh, indices, weights, K: int, force_shape_i
         return _check(_lib.exl3b_mgemm(
             _stream(A), _ptr(A), _ptr(B), _ptr(C), _ptr(suh), _ptr(A_had), _ptr(svh),
             _ptr(indices), num_indices, _ptr(weights),
-            bszm_in, bszm_out, m, k, n, int(K), _cb(mcg, mul1), int(c_fp32),
+            bszm_in, bszm_out, m, k, n, int(K), cb, int(c_fp32),
             int(min_index), int(max_index), int(num_tokens),
             _ptr(size_n_list), _ptr(c_ptrs), num_c_ptrs, int(force_shape_idx), int(force_num_sms)))
 
@@ -576,7 +569,7 @@ def reconstruct_slice(unpacked, packed, K: int, mcg, mul1, n_offset: int) -> Non
     if packed.shape[2] != 256 * K // 16:
         raise RuntimeError("packed: incorrect size in dimension 2")
     _dtype(unpacked, torch.half, "unpacked")
-    assert unpacked.is_contiguous() and packed.is_contiguous()
+    _contiguous("reconstruct", unpacked, packed)
     with torch.cuda.device(unpacked.device):
         _check(_lib.exl3b_reconstruct(_stream(unpacked), _ptr(unpacked), _ptr(packed), unpacked.shape[0],
                                       unpacked.shape[1], packed.shape[1], int(K), _cb(mcg, mul1), int(n_offset)))
@@ -601,7 +594,7 @@ def reconstruct_had_slice(unpacked, packed, suh, svh, K: int, mcg, mul1, n_offse
         raise RuntimeError("reconstruct_had: suh size")
     if svh.numel() < unpacked.shape[1]:
         raise RuntimeError("reconstruct_had: svh size")
-    assert unpacked.is_contiguous() and packed.is_contiguous()
+    _contiguous("reconstruct_had", unpacked, packed)
     with torch.cuda.device(unpacked.device):
         _check(_lib.exl3b_reconstruct_had(_stream(unpacked), _ptr(unpacked), _ptr(packed), _ptr(suh), _ptr(svh),
                                           unpacked.shape[0], unpacked.shape[1], packed.shape[1], int(K),
@@ -621,7 +614,7 @@ def had_r_128(input, output, pre_scale, post_scale, scale: float) -> None:
         _dtype(output, torch.float, "output"); fp32 = 1
     else:
         raise RuntimeError("unsupported datatype")
-    assert input.is_contiguous() and output.is_contiguous()
+    _contiguous("had_r_128", input, output)
     with torch.cuda.device(input.device):
         _check(_lib.exl3b_had_r_128(_stream(input), _ptr(input), _ptr(output), _ptr(pre_scale), _ptr(post_scale),
                                     float(scale), input.shape[0], input.shape[1], fp32))
@@ -642,7 +635,7 @@ def hgemm(a, b, c) -> None:
         raise RuntimeError("a, b and c incompatible shapes")
     if c.stride(-1) != 1:
         raise RuntimeError("c must have contiguous columns")
-    assert a.is_contiguous() and b.is_contiguous()
+    _contiguous("hgemm", a, b)
     with torch.cuda.device(a.device):
         _check(_lib.exl3b_hgemm(_stream(a), _ptr(a), _ptr(b), _ptr(c), m, k, n, int(c.dtype == torch.float),
                                 c.stride(-2)))
@@ -656,14 +649,11 @@ def exl3_gemv(A, B, C, suh, A_had, svh, mcg, mul1) -> None:
     tensor-core decode-GEMM is the small-m kernel -- so the same eligibility rules are enforced and the call is exl3_gemm.
     """
     _need_cuda(A, B, C, suh, A_had, svh)
-    if B.dim() != 3:
-        raise RuntimeError("B: incorrect number of dimensions, must be 3")
+    _dtype(A, torch.half, "A")
+    m, k, n, K, _ = _gemm_operands("exl3_gemv", A, B, C)
     if suh is None or A_had is None or svh is None:
         raise RuntimeError("exl3_gemv requires suh, A_had and svh")
-    size_k = A.shape[-1]
-    size_m = A.numel() // size_k if size_k else 0
-    size_n, K = B.shape[1] * 16, B.shape[2] // 16
-    if not (1 <= size_m <= 8 and 2 <= K <= 4 and size_k % 128 == 0 and size_n % 128 == 0):
+    if not (1 <= m <= 8 and 2 <= K <= 4 and k % 128 == 0 and n % 128 == 0):
         raise RuntimeError("exl3_gemv: call not eligible (needs m <= 8, K in 2..4, k % 128 == 0, n % 128 == 0)")
     exl3_gemm(A, B, C, suh, A_had, svh, -1, mcg, mul1, 0)
 
@@ -777,32 +767,17 @@ def exl3_gemm_gated(G, U, B, C, suh, svh, act: int, act_limit: float, mcg, mul1,
     on the same path and grid: tag 210 for mul1 at m <= 4, tag 200 otherwise (include/exl3b200.h).  Returns the path tag.
     """
     _need_cuda(G, U, B, C, suh, svh)
-    if B.dim() != 3:
-        raise RuntimeError("B: incorrect number of dimensions, must be 3")
-    _dtype(B, torch.int16, "B")
     if G.dtype == torch.float:
         _dtype(U, torch.float, "U")
     else:
         _dtype(G, torch.half, "G")
         _dtype(U, torch.half, "U")
-    c_fp32 = C.dtype == torch.float
-    if not c_fp32:
-        _dtype(C, torch.half, "C")
-    size_k = G.shape[-1]
-    size_m = G.numel() // size_k if size_k else 0
-    size_n = B.shape[1] * 16
     if U.shape != G.shape:
         raise RuntimeError("G and U incompatible shapes")
-    if size_k != B.shape[0] * 16:
-        raise RuntimeError("G and B incompatible shapes")
-    if C.shape[-1] != size_n or C.numel() != size_m * size_n:
-        raise RuntimeError("C and B incompatible shapes")
-    if not (G.is_contiguous() and U.is_contiguous() and B.is_contiguous() and C.is_contiguous()):
-        raise RuntimeError("exl3_gemm_gated: tensors must be contiguous")
-    K = B.shape[2] // 16
+    m, k, n, K, c_fp32 = _gemm_operands("exl3_gemm_gated", G, B, C, U, c_numel=True, a_name="G")
     with torch.cuda.device(G.device):
         return _check(_lib.exl3b_gemm_gated(
-            _stream(G), _ptr(G), _ptr(U), _ptr(B), _ptr(C), _ptr(suh), _ptr(svh), size_m, size_k, size_n, K, _cb(mcg, mul1),
+            _stream(G), _ptr(G), _ptr(U), _ptr(B), _ptr(C), _ptr(suh), _ptr(svh), m, k, n, K, _cb(mcg, mul1),
             int(c_fp32), int(G.dtype == torch.float), int(act), float(act_limit), int(force_num_sms)))
 
 
