@@ -22,7 +22,7 @@
 //     halves, of k-tile 4r + c (r = 0, 1).  Its 2 x 16 products ARE the wgmma A fragments (rows chunk / chunk + 8, K slots
 //     c / c + 4) of 8 wgmma.m64nNk32 per r; the K order inside each instruction is permuted accordingly in the digit tile.
 //     int32 accumulators stay in registers for a sub-segment and are then handed to the epilogue through shared memory
-//   * a CTA prologue (warps 2..19, redundantly per CTA) transforms the rows once into a shared-memory cache and finds the
+//   * a CTA prologue (warps 1..23, redundantly per CTA) transforms the rows once into a shared-memory cache and finds the
 //     per-row |xh| maximum; the two transform warps then write per-unit activation digits + digit sums
 //   * split-K partial sums travel through a sentinel-armed exchange buffer: contributors store and leave, the CTA owning the
 //     strip's first k-segment (it processes it last) adds them to its registers in fixed CTA order and re-arms the slots --
@@ -33,8 +33,14 @@
 #pragma once
 #include "i8_pipeline.cuh"
 #include "act.cuh"
+#include <type_traits>
 
 namespace exl3b {
+
+// (row, k-block) input loads a prologue warp keeps in flight per round trip: 2 registers each, plus 2 per block for suh.
+// 5 covers k = 23 * 5 * 128 = 14720 (Llama's down projection) at m = 1 in one round trip; more blocks per round trip made
+// ptxas spill in the routed kernel, whose spill-free register allocation is kept (ptxas -v).
+constexpr int I8_PRO_SLOTS = 5;
 
 __host__ __device__ inline TcSmemLayout i8_smem_layout(int K, int MR, int stages, int cache_bytes)
 {
@@ -214,77 +220,68 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         if (lane == 0) atomicMax(&s_absmax[r], __float_as_uint(mx));
     };
 
-    // ---- prologue: per-row max |xh| over the whole row (warps 2..19), overlapped with the first weight loads ----
-    if (warp == 0)
+    // ---- prologue: per-row max |xh| over the whole row (every warp but the producer), overlapped with the first weight loads ----
+    // The decode warps can start only after it, so it is on every launch's critical path, and its cost is the number of
+    // dependent memory round trips.  Warp w (1..23) takes the k-blocks w - 1, w - 1 + 23, ... with all rows of each block and
+    // issues the loads of up to I8_PRO_SLOTS (row, block) pairs before its first Hadamard: at m = 1 that is one round trip up
+    // to k = 23 * I8_PRO_SLOTS * 128.  suh is a weight (it does not depend on the previous kernel) and usually comes from DRAM: the first
+    // round's blocks are fetched BEFORE griddepcontrol.wait, the activations only after it.  The epilogue warps take part too;
+    // their pdl_wait here comes before their first use of A.
+    if (warp != 0)
     {
-        // producer starts streaming weights immediately (below); it does not take part in the prologue
-    }
-    if (warp >= TC_XF_WARP0 && warp < TC_EPI_WARP0)
-    {
-        const int nw = TC_EPI_WARP0 - TC_XF_WARP0;       // 18 warps
-        if constexpr (MR <= 4)
+        constexpr int nw = TC_THREADS / 32 - 1;
+        const int w0 = warp - 1;
+        auto transform = [&](auto rows)
         {
-            // Two tasks (row, k-block) per step with both loads in flight together, and the suh blocks of the first step fetched
-            // BEFORE griddepcontrol.wait: suh is a weight (it does not depend on the previous kernel) and usually comes from
-            // DRAM, the activations come from L2 -- one DRAM latency and one L2 latency less on every launch's critical path.
-            const int T = p.m * KB, w0 = warp - TC_XF_WARP0;
-            uint2 sc0 = make_uint2(0, 0), sc1 = make_uint2(0, 0);
-            if (suh)
+            constexpr int M = decltype(rows)::value;     // rows loaded per block: the register arrays are sized for M
+            constexpr int NB = I8_PRO_SLOTS / M > 0 ? I8_PRO_SLOTS / M : 1;
+            uint2 sc[NB];
+            auto load_suh = [&](int kb0)
             {
-                if (w0 < T) sc0 = *reinterpret_cast<const uint2*>(suh + (w0 % KB) * 128 + lane * 4);
-                if (w0 + nw < T) sc1 = *reinterpret_cast<const uint2*>(suh + ((w0 + nw) % KB) * 128 + lane * 4);
-            }
+                #pragma unroll
+                for (int j = 0; j < NB; ++j)
+                {
+                    const int kb = kb0 + j * nw;
+                    sc[j] = make_uint2(0, 0);
+                    if (suh && kb < KB) sc[j] = *reinterpret_cast<const uint2*>(suh + kb * 128 + lane * 4);
+                }
+            };
+            load_suh(w0);
             if constexpr (!ROUTED) pdl_wait();            // A is produced by the previous kernel (ROUTED waited at the top)
-            for (int task = w0; task < T; task += 2 * nw)
+            for (int kb0 = w0; kb0 < KB; kb0 += NB * nw)
             {
-                const int ta = task, tb = task + nw;
-                const int ra = ta / KB, ka = ta % KB, rb = tb / KB, kb_ = tb % KB;
-                if (task != w0 && suh)
-                {
-                    sc0 = *reinterpret_cast<const uint2*>(suh + ka * 128 + lane * 4);
-                    if (tb < T) sc1 = *reinterpret_cast<const uint2*>(suh + kb_ * 128 + lane * 4);
-                }
-                const uint2 raw0 = raw_block(ra, ka);
-                uint2 raw1 = make_uint2(0, 0);
-                if (tb < T) raw1 = raw_block(rb, kb_);
-                float v[4];
-                xh_finish(raw0, sc0, v);
-                xh_publish(ra, ka, v);
-                if (tb < T)
-                {
-                    xh_finish(raw1, sc1, v);
-                    xh_publish(rb, kb_, v);
-                }
-            }
-        }
-        else
-        {
-            pdl_wait();                                   // A is produced by the previous kernel
-            // up to 8 rows: one k-block of ALL rows per step, the rows' loads in flight together (one L2 round trip per step
-            // instead of one per row)
-            for (int kb = warp - TC_XF_WARP0; kb < KB; kb += nw)
-            {
-                uint2 scb = make_uint2(0, 0), raw[MR];
-                if (suh) scb = *reinterpret_cast<const uint2*>(suh + kb * 128 + lane * 4);
+                if (kb0 != w0) load_suh(kb0);
+                uint2 raw[NB][M];
                 #pragma unroll
-                for (int r = 0; r < MR; ++r)
+                for (int j = 0; j < NB; ++j)
                 {
-                    raw[r] = make_uint2(0, 0);
-                    if (r < p.m) raw[r] = raw_block(r, kb);
-                }
-                #pragma unroll
-                for (int r = 0; r < MR; ++r)
-                {
-                    if (r < p.m)
+                    #pragma unroll
+                    for (int r = 0; r < M; ++r)
                     {
-                        float v[4];
-                        xh_finish(raw[r], scb, v);
-                        xh_publish(r, kb, v);
+                        raw[j][r] = make_uint2(0, 0);
+                        if (kb0 + j * nw < KB && r < p.m) raw[j][r] = raw_block(r, kb0 + j * nw);
+                    }
+                }
+                #pragma unroll
+                for (int j = 0; j < NB; ++j)
+                {
+                    #pragma unroll
+                    for (int r = 0; r < M; ++r)
+                    {
+                        if (kb0 + j * nw < KB && r < p.m)
+                        {
+                            float v[4];
+                            xh_finish(raw[j][r], sc[j], v);
+                            xh_publish(r, kb0 + j * nw, v);
+                        }
                     }
                 }
             }
-        }
-        asm volatile("bar.sync 2, %0;" :: "n"((TC_EPI_WARP0 - TC_XF_WARP0) * 32) : "memory");
+        };
+        // batch 1 (the decode token) gets the widest round trip; otherwise the arrays are sized for MR rows
+        if (p.m == 1) transform(std::integral_constant<int, 1>());
+        else transform(std::integral_constant<int, MR>());
+        asm volatile("bar.sync 2, %0;" :: "n"(TC_THREADS - 32) : "memory");
         if (warp == TC_DEC_WARP0 && lane == 0) stamp(2);
     }
 
@@ -379,6 +376,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
                 if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) stamp(3);
                 const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
                 mbar_wait(X_FULL(s), sph);                                   // the unit's activation digits
+                if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) stamp(4);
                 const int* dsum = reinterpret_cast<const int*>(smem + L.off_b + s * L.b_bytes + I8_B_BYTES);
                 if (c < p.m) t_lo += dsum[c];
                 if (MR > 4 && c + 4 < p.m) t_hi += dsum[c + 4];

@@ -4,16 +4,24 @@ Phase split of the int8 decode-GEMM (tag 210) launches of the flagship token, fr
 bring-up build:
 
     EXL3B_LIB_SUFFIX=_dbg EXL3B_TC_DEBUG=1 python -m exllamav3_b200.build
-    python tools/i8_phase_profile.py --library exllamav3_b200/libexl3b200_dbg.so [--reps 20] [--out FILE]
+    python tools/i8_phase_profile.py --library exllamav3_b200/libexl3b200_dbg.so [--reps 20] [--replay] [--out FILE]
 
-Runs the launches of one Llama-3.1-8B layer as bench.py issues them (q+k+v fan-out, o, gate+up exl3_mgemm, down) and the
-lm_head, each `reps` times after a warm-up, with the timeline buffer set (exl3b_debug_tc_timeline).  Per CTA it splits a
-launch into
-    ramp    kernel start -> the first decode warp has its first unit's weights   (stamps 0 -> 3)
-    steady  decode and MMA of the CTA's units, up to the last unit's MMAs        (stamps 3 -> 10)
-    tail    epilogue and split-K exchange                                         (stamps 10 -> 8)
+Default (isolated): runs the launches of one Llama-3.1-8B layer as bench.py issues them (q+k+v fan-out, o, gate+up
+exl3_mgemm, down) and the lm_head, each `reps` times after a warm-up, each launch alone after a synchronize, with the
+timeline buffer set (exl3b_debug_tc_timeline).  Per CTA it splits a launch into
+    ramp      kernel start -> the first decode warp has its first unit's weights   (stamps 0 -> 3)
+      prologue  kernel start -> end of the CTA's row transform (bar.sync 2)        (stamps 0 -> 2)
+      digits    prologue end -> the first unit's activation digits (X_FULL)       (stamps 2 -> 4)
+    steady    decode and MMA of the CTA's units, up to the last unit's MMAs        (stamps 3 -> 10)
+    tail      epilogue and split-K exchange                                         (stamps 10 -> 8)
 and prints one JSON line per launch with the median and the max over CTAs (pooled over the repetitions), in microseconds
 (%globaltimer), plus the steady time per unit: the median steady time over the mean units per CTA.
+
+--replay: what a launch costs between its predecessor and its first MMA inside the token, where PDL lets a launch start
+before the previous one ends.  Captures two layers' launches and the lm_head into one CUDA graph exactly as bench.py issues
+them (each launch with its own timeline buffer), replays it `reps` times, and reports for the second layer's launches and
+the lm_head the boundary: this launch's first X_FULL per CTA (stamp 4) minus the previous launch's last CTA end (the
+maximum of stamp 8 over its CTAs); median and max over CTAs, pooled over the replays.  %globaltimer is one clock per GPU.
 """
 from __future__ import annotations
 import argparse, ctypes, json, os, statistics, subprocess, sys
@@ -22,10 +30,100 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SLOTS = 64                                       # u64 stamps per CTA (gemm_tc_i8_body.cuh: p.dbg[blockIdx.x * 64 + slot])
 
 
+def q(v):
+    return {"median": round(statistics.median(v), 2), "max": round(max(v), 2)}
+
+
+def launch_name(ln):
+    return "+".join(m["name"] for m in ln["mats"])
+
+
+def isolated(tok, ext, buf, reps, library):
+    import torch
+    results = []
+    for ln in tok.launches:
+        mats = ln["mats"]
+        units = sum((m["k"] // 128) * (m["n"] // 128) for m in mats)
+        for _ in range(3):
+            tok.run([ln])
+        torch.cuda.synchronize()
+        ph = {k: [] for k in ("ramp", "prologue", "digits", "steady", "tail", "total")}
+        ctas = []
+        ext.lib.exl3b_debug_tc_timeline(ctypes.c_void_p(buf.data_ptr()))
+        try:
+            for _ in range(reps):
+                buf.zero_()
+                tok.run([ln])
+                torch.cuda.synchronize()
+                rows = [r for r in buf.cpu().tolist() if r[0] and r[2] and r[3] and r[4] and r[10] and r[8]]
+                ctas.append(len(rows))
+                for r in rows:
+                    ph["ramp"].append((r[3] - r[0]) / 1e3)
+                    ph["prologue"].append((r[2] - r[0]) / 1e3)
+                    ph["digits"].append((r[4] - r[2]) / 1e3)
+                    ph["steady"].append((r[10] - r[3]) / 1e3)
+                    ph["tail"].append((r[8] - r[10]) / 1e3)
+                    ph["total"].append((r[8] - r[0]) / 1e3)
+        finally:
+            ext.lib.exl3b_debug_tc_timeline(ctypes.c_void_p(0))
+        torch.cuda.synchronize()
+        assert ph["ramp"], f"{launch_name(ln)}: no timeline stamps (is {library} the EXL3B_TC_DEBUG build?)"
+        n_cta = statistics.median(ctas)
+        res = {"launch": launch_name(ln), "k": mats[0]["k"], "n": [m["n"] for m in mats], "K": mats[0]["K"], "units": units,
+               "ctas": n_cta, "ramp_us": q(ph["ramp"]), "prologue_us": q(ph["prologue"]), "digits_us": q(ph["digits"]),
+               "steady_us": q(ph["steady"]), "tail_us": q(ph["tail"]), "cta_total_us": q(ph["total"]),
+               "steady_us_per_unit": round(statistics.median(ph["steady"]) / (units / n_cta), 3)}
+        results.append(res)
+        print(json.dumps(res), flush=True)
+    return results
+
+
+def replay(tok, ext, num_sms, reps):
+    import torch
+    launches = tok.launches
+    bufs = [torch.zeros((4 * num_sms, SLOTS), dtype=torch.int64, device=tok.dev) for _ in launches]
+    stream = torch.cuda.Stream()
+    with torch.cuda.stream(stream):
+        for _ in range(3):
+            tok.run()
+    stream.synchronize()
+    graph = torch.cuda.CUDAGraph()
+    try:
+        with torch.cuda.graph(graph, stream=stream):
+            for ln, b in zip(launches, bufs):      # the buffer address is a kernel argument, set per launch at capture
+                ext.lib.exl3b_debug_tc_timeline(ctypes.c_void_p(b.data_ptr()))
+                tok.run([ln])
+    finally:
+        ext.lib.exl3b_debug_tc_timeline(ctypes.c_void_p(0))
+    first = len(launches) - 5                      # the last layer's four launches and the lm_head
+    bound = {i: [] for i in range(first, len(launches))}
+    for _ in range(reps + 2):
+        with torch.cuda.stream(stream):
+            for b in bufs:
+                b.zero_()
+            graph.replay()
+        stream.synchronize()
+        st = [b.cpu().tolist() for b in bufs]
+        if _ < 2:                                  # warm-up replays
+            continue
+        for i in bound:
+            prev_end = max(r[8] for r in st[i - 1] if r[8])
+            bound[i] += [(r[4] - prev_end) / 1e3 for r in st[i] if r[4]]
+    del graph
+    results = []
+    for i, v in bound.items():
+        assert v, f"{launch_name(launches[i])}: no timeline stamps"
+        res = {"launch": launch_name(launches[i]), "after": launch_name(launches[i - 1]), "boundary_us": q(v)}
+        results.append(res)
+        print(json.dumps(res), flush=True)
+    return results
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--library", required=True, help="bring-up build of libexl3b200 (EXL3B_TC_DEBUG)")
     ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--replay", action="store_true", help="boundary times inside a replayed CUDA graph of the token's launches")
     ap.add_argument("--out", default=None, help="also write the results (JSON) here")
     args = ap.parse_args()
     os.environ["EXL3B_LIBRARY"] = os.path.abspath(args.library)
@@ -36,51 +134,23 @@ def main():
 
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
-    cfg = dict(bench.MODELS["llama-3.1-8b"], layers=1)
+    cfg = dict(bench.MODELS["llama-3.1-8b"], layers=2 if args.replay else 1)
     tok = bench.Token(cfg, 1, 0, dev)
     num_sms = torch.cuda.get_device_properties(dev).multi_processor_count
-    buf = torch.zeros((4 * num_sms, SLOTS), dtype=torch.int64, device=dev)
-    results = []
-    for ln in tok.launches:
-        mats = ln["mats"]
-        name = "+".join(m["name"] for m in mats)
-        units = sum((m["k"] // 128) * (m["n"] // 128) for m in mats)
-        for _ in range(3):
-            tok.run([ln])
-        torch.cuda.synchronize()
-        ramp, steady, tail, total, ctas = [], [], [], [], []
-        ext.lib.exl3b_debug_tc_timeline(ctypes.c_void_p(buf.data_ptr()))
-        try:
-            for _ in range(args.reps):
-                buf.zero_()
-                tok.run([ln])
-                torch.cuda.synchronize()
-                st = buf.cpu()
-                rows = [r for r in st.tolist() if r[0] and r[3] and r[10] and r[8]]
-                ctas.append(len(rows))
-                for r in rows:
-                    ramp.append((r[3] - r[0]) / 1e3)
-                    steady.append((r[10] - r[3]) / 1e3)
-                    tail.append((r[8] - r[10]) / 1e3)
-                    total.append((r[8] - r[0]) / 1e3)
-        finally:
-            ext.lib.exl3b_debug_tc_timeline(ctypes.c_void_p(0))
-        torch.cuda.synchronize()
-        assert ramp, f"{name}: no timeline stamps (is {args.library} the EXL3B_TC_DEBUG build?)"
-        n_cta = statistics.median(ctas)
-        q = lambda v: {"median": round(statistics.median(v), 2), "max": round(max(v), 2)}
-        res = {"launch": name, "k": mats[0]["k"], "n": [m["n"] for m in mats], "K": mats[0]["K"], "units": units,
-               "ctas": n_cta, "ramp_us": q(ramp), "steady_us": q(steady), "tail_us": q(tail), "cta_total_us": q(total),
-               "steady_us_per_unit": round(statistics.median(steady) / (units / n_cta), 3)}
-        results.append(res)
-        print(json.dumps(res), flush=True)
+    if args.replay:
+        results = replay(tok, ext, num_sms, args.reps)
+    else:
+        buf = torch.zeros((4 * num_sms, SLOTS), dtype=torch.int64, device=dev)
+        results = isolated(tok, ext, buf, args.reps, args.library)
     gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
-    print(json.dumps({"gpu": gpu, "library": os.path.basename(args.library)}), flush=True)
+    print(json.dumps({"gpu": gpu, "library": os.path.basename(args.library), "mode": "replay" if args.replay else "isolated"}),
+          flush=True)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
-            json.dump({"gpu": gpu, "library": os.path.basename(args.library), "launches": results}, f, indent=1)
+            json.dump({"gpu": gpu, "library": os.path.basename(args.library), "mode": "replay" if args.replay else "isolated",
+                       "launches": results}, f, indent=1)
 
 
 if __name__ == "__main__":
