@@ -187,7 +187,8 @@ __device__ __forceinline__ void group_unit(const ChainCtx& cx, int tl, int lane,
     CH_STAMP(tr, 2);
     const uint8_t* b = cx.smem + cx.L.off_b + s * i8_b_stage(CH_MR);
     if (c < m) tsum += *reinterpret_cast<const int*>(b + i8_b_bytes(CH_MR) + 4 * c);
-    i8_unit_mma<K, CH_MR>(reinterpret_cast<const uint32_t*>(cx.smem + s * cx.w_bytes), smem_desc(smem_u32(b), 128, 4096, 0), tl, lane, acc);
+    I8BatchClock clk{};
+    i8_unit_mma<K, CH_MR>(reinterpret_cast<const uint32_t*>(cx.smem + s * cx.w_bytes), smem_desc(smem_u32(b), 128, 4096, 0), tl, lane, acc, clk);
     CH_STAMP(tr, 3);
     __syncwarp();
     if (lane == 0) mbar_arrive(cx.W_EMPTY(s));

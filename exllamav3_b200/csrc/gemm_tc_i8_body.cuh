@@ -130,9 +130,10 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
 
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
     const uint32_t bar0 = smem_u32(bars);
+    // W_FULL(s): the unit's weights (TMA bytes) AND its activation digits (the digit warp's arrival), so that a decode warp
+    // takes one barrier per unit
     auto W_FULL = [&](int s) { return bar0 + 8u * s; };
     auto W_EMPTY = [&](int s) { return bar0 + 8u * (S + s); };
-    auto X_FULL = [&](int s) { return bar0 + 8u * (2 * S + s); };
     auto D_FULL = [&](int s) { return bar0 + 8u * (3 * S + 8 + s); };
     auto D_EMPTY = [&](int s) { return bar0 + 8u * (3 * S + 10 + s); };
     uint32_t* misc = reinterpret_cast<uint32_t*>(smem + L.off_bars + 8 * (3 * TC_MAX_STAGES + 16));
@@ -160,8 +161,9 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     if (warp == 0)
     {
         // one barrier per lane and round instead of ~60 serial initialisations by one thread
-        // W_EMPTY: the eight decode warps of the unit's group, after their MMAs have read the weights' digit tile
-        for (int s = lane; s < S; s += 32) { mbar_init(W_FULL(s), 1); mbar_init(X_FULL(s), 1); mbar_init(W_EMPTY(s), TC_DEC_WARPS / I8_DEC_GROUPS); }
+        // W_FULL: the producer (expect_tx) and the unit's digit warp; W_EMPTY: the eight decode warps of the unit's group, after
+        // their MMAs have read the weights and the digit tile
+        for (int s = lane; s < S; s += 32) { mbar_init(W_FULL(s), 2); mbar_init(W_EMPTY(s), TC_DEC_WARPS / I8_DEC_GROUPS); }
         if (lane < 2) { mbar_init(D_FULL(lane), TC_DEC_WARPS); mbar_init(D_EMPTY(lane), 4); }
         else if (lane < 2 + MR) s_absmax[lane - 2] = 0u;
         fence_barrier_init();
@@ -329,7 +331,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         {
             I8_WAITCNT(wf_a, W_EMPTY(s), ph ^ 1);
             mbar_wait<64>(W_EMPTY(s), ph ^ 1);
-            i8_write_digit_tile<MR>(smem + L.off_b + s * L.b_bytes, inv_scale, p.m, lane, X_FULL(s), [&](int r, float (&v)[4])
+            i8_write_digit_tile<MR>(smem + L.off_b + s * L.b_bytes, inv_scale, p.m, lane, W_FULL(s), [&](int r, float (&v)[4])
             {
                 if (cached)
                 {
@@ -360,6 +362,12 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         #pragma unroll
         for (int i = 0; i < MR; ++i) acc[i] = 0u;
         int t_lo = 0, t_hi = 0;                          // digit sums of activation rows c and c + 4 over the group's units
+        // debug timeline: lane 0 of the group's first warp stamps its first 16 batches into slots 16 + 16 g ..
+        I8BatchClock clk{};
+#ifdef EXL3B_TC_DEBUG
+        unsigned long long* const dbg_row = p.dbg && nh == 0 && wq == 0 && lane == 0 ? p.dbg + blockIdx.x * 64 : nullptr;
+        clk.dbg = dbg_row ? dbg_row + 16 + 16 * g : nullptr;
+#endif
         int s = 0, sph = 0, dbuf = 0, dphase = 0, seg_left = 0, sub_left = 0;
         int kb = ubeg % KB;
         for (int u = 0; u < n_units; ++u)
@@ -372,15 +380,24 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             if (sub_left == 0) sub_left = seg_left < I8_SUB_UNITS ? seg_left : I8_SUB_UNITS;
             if ((u & 1) == g)
             {
-                mbar_wait<32>(W_FULL(s), sph);
-                if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) stamp(3);
+#ifdef EXL3B_TC_DEBUG
+                uint32_t t_in; asm volatile("mov.u32 %0, %%clock;" : "=r"(t_in) :: "memory");
+#endif
+                mbar_wait<32>(W_FULL(s), sph);                               // the unit's weights and activation digits
+                if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) { stamp(3); stamp(4); }
                 const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
-                mbar_wait(X_FULL(s), sph);                                   // the unit's activation digits
-                if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) stamp(4);
+#ifdef EXL3B_TC_DEBUG
+                // slots 48 + 4 g + j: SM clock before (low word) and after (high word) the wait of the group's unit j < 4
+                if (dbg_row && (u >> 1) < 4)
+                {
+                    uint32_t t_out; asm volatile("mov.u32 %0, %%clock;" : "=r"(t_out) :: "memory");
+                    dbg_row[48 + 4 * g + (u >> 1)] = ((unsigned long long) t_out << 32) | t_in;
+                }
+#endif
                 const int* dsum = reinterpret_cast<const int*>(smem + L.off_b + s * L.b_bytes + I8_B_BYTES);
                 if (c < p.m) t_lo += dsum[c];
                 if (MR > 4 && c + 4 < p.m) t_hi += dsum[c + 4];
-                i8_unit_mma<K, MR>(wst, desc0 + (uint64_t) ((s * L.b_bytes) >> 4), tl, lane, acc);
+                i8_unit_mma<K, MR>(wst, desc0 + (uint64_t) ((s * L.b_bytes) >> 4), tl, lane, acc, clk);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(W_EMPTY(s));
                 if (u == n_units - 1 && wq == 0 && lane == 0) stamp(10);

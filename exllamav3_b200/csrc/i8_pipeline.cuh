@@ -35,7 +35,7 @@ __host__ __device__ constexpr int i8_d_bytes(int MR) { return 2 * 2 * 128 * 2 * 
 // Digit tile of one unit, written by one activation warp into the stage's tile at `dst`: row_values(r, v) gives lane's four
 // transformed values k = 4 lane .. 4 lane + 3 of row r < m.  Each value becomes two digits replicated over the 4 product bytes,
 // stored in the wgmma K order; the per-row digit sums go behind the tile.  Then the tile is made visible to the async proxy and
-// the warp arrives on the stage's X_FULL barrier.
+// the warp arrives on `x_full` (the chain kernel's X_FULL; in the single-GEMM body the stage's W_FULL, which also takes the weights).
 template <int MR, typename RowValues>
 __device__ __forceinline__ void i8_write_digit_tile(uint8_t* dst, const float (&inv_scale)[MR], int m, int lane, uint32_t x_full,
                                                     RowValues&& row_values)
@@ -87,11 +87,33 @@ __device__ __forceinline__ void i8_write_digit_tile(uint8_t* dst, const float (&
     if (lane == 0) mbar_arrive(x_full);
 }
 
+// Timeline of a decode warp's k-half wgmma batches in the EXL3B_TC_DEBUG build (tools/i8_phase_profile.py): the SM clock at
+// the issue and at the retirement of each batch.  The other builds keep no state and emit nothing.
+struct I8BatchClock
+{
+#ifdef EXL3B_TC_DEBUG
+    unsigned long long* dbg;                 // slots of the CTA's timeline row (16 batches), null: no stamps
+    int i;                                   // next batch
+    uint32_t t_issue;
+    __device__ __forceinline__ void issue() { asm volatile("mov.u32 %0, %%clock;" : "=r"(t_issue) :: "memory"); }
+    __device__ __forceinline__ void retired()
+    {
+        uint32_t t; asm volatile("mov.u32 %0, %%clock;" : "=r"(t) :: "memory");
+        if (dbg && i < 16) dbg[i] = ((unsigned long long) t << 32) | t_issue;          // retirement (high word), issue (low)
+        ++i;
+    }
+#else
+    __device__ __forceinline__ void issue() {}
+    __device__ __forceinline__ void retired() {}
+#endif
+};
+
 // One unit (128 k x 128 n weights) of a decode warp: lane (chunk, c) decodes tile column `tl`, both halves, of k-tile 4 r + c
 // (r = 0, 1) from the weight stage `wst` straight into wgmma A fragments, 8 wgmma.m64nNk32 per r against the digit tile at
-// `desc_s`, into acc.  The caller has waited for both the weights and the digits.
+// `desc_s`, into acc.  The caller has waited for both the weights and the digits.  `clk` takes the batches' issue and
+// retirement times (debug timeline).
 template <int K, int MR>
-__device__ __forceinline__ void i8_unit_mma(const uint32_t* wst, uint64_t desc_s, int tl, int lane, uint32_t (&acc)[MR])
+__device__ __forceinline__ void i8_unit_mma(const uint32_t* wst, uint64_t desc_s, int tl, int lane, uint32_t (&acc)[MR], I8BatchClock& clk)
 {
     const int chunk = lane >> 2, c = lane & 3;
     #pragma unroll
@@ -104,12 +126,14 @@ __device__ __forceinline__ void i8_unit_mma(const uint32_t* wst, uint64_t desc_s
         decode16_i8<K, 1>(w, o1);
         #pragma unroll
         for (int i = 0; i < MR; ++i) reg_fence(acc[i]);
+        clk.issue();
         wgmma_fence();
         #pragma unroll
         for (int j = 0; j < 8; ++j)
             wgmma_u8s8<MR>(acc, o0[2 * j], o1[2 * j], o0[2 * j + 1], o1[2 * j + 1], desc_s + (uint64_t) (16 * (8 * r + j)));
         wgmma_commit();
         wgmma_wait<0>();
+        clk.retired();
         #pragma unroll
         for (int i = 0; i < 16; ++i) { reg_fence(o0[i]); reg_fence(o1[i]); }
         #pragma unroll

@@ -11,16 +11,21 @@ exl3_mgemm, down) and the lm_head, each `reps` times after a warm-up, each launc
 timeline buffer set (exl3b_debug_tc_timeline).  Per CTA it splits a launch into
     ramp      kernel start -> the first decode warp has its first unit's weights   (stamps 0 -> 3)
       prologue  kernel start -> end of the CTA's row transform (bar.sync 2)        (stamps 0 -> 2)
-      digits    prologue end -> the first unit's activation digits (X_FULL)       (stamps 2 -> 4)
+      digits    prologue end -> the first unit's weights and digits (W_FULL)      (stamps 2 -> 4)
     steady    decode and MMA of the CTA's units, up to the last unit's MMAs        (stamps 3 -> 10)
     tail      epilogue and split-K exchange                                         (stamps 10 -> 8)
 and prints one JSON line per launch with the median and the max over CTAs (pooled over the repetitions), in microseconds
-(%globaltimer), plus the steady time per unit: the median steady time over the mean units per CTA.
+(%globaltimer), plus the steady time per unit: the median steady time over the mean units per CTA.  Under "turns" it shows how
+the two decode groups' k-half wgmma batches lie against each other, from the SM clock (%clock) at the issue and the retirement
+of the first 16 batches of one warp per group (slots 16-47, see turn_stats): the issue offset between the groups, the share of
+batches (and of batch time) during which the other group also had a batch in flight, the batch time, the gaps between batches
+inside a unit and between units, and the cycle per k-half; unit_wait_clk is the decode group's wait for a unit's weights and
+digits (slots 48-55).  The decode warps' stamps are SM clocks: one clock per SM, compared only inside a CTA.
 
 --replay: what a launch costs between its predecessor and its first MMA inside the token, where PDL lets a launch start
 before the previous one ends.  Captures two layers' launches and the lm_head into one CUDA graph exactly as bench.py issues
 them (each launch with its own timeline buffer), replays it `reps` times, and reports for the second layer's launches and
-the lm_head the boundary: this launch's first X_FULL per CTA (stamp 4) minus the previous launch's last CTA end (the
+the lm_head the boundary: this launch's first W_FULL per CTA (stamp 4) minus the previous launch's last CTA end (the
 maximum of stamp 8 over its CTAs); median and max over CTAs, pooled over the replays.  %globaltimer is one clock per GPU.
 """
 from __future__ import annotations
@@ -38,6 +43,66 @@ def launch_name(ln):
     return "+".join(m["name"] for m in ln["mats"])
 
 
+def batch_windows(row, g):
+    """(issue, retire) SM clocks of decode group g's first k-half batches in one CTA's timeline row (slots 16 + 16 g + i)."""
+    out = []
+    for v in row[16 + 16 * g: 32 + 16 * g]:
+        if not v:
+            break
+        v &= (1 << 64) - 1
+        out.append((v & 0xffffffff, v >> 32))
+    return out
+
+
+def turn_stats(rows):
+    """How the two decode groups' wgmma batches lie against each other, from the batch windows of one warp per group:
+    offset = group 1's i-th issue minus group 0's i-th issue (clocks), overlap_batches = share of batches during more than
+    half of whose issue -> retire window the other group also had a batch in flight, overlap_time = the same as a share of
+    all batch time, batch = issue -> retire, gap = retire of k-half 0 -> issue of k-half 1 of the same unit (the decode of
+    a k-half), unit_gap = retire of k-half 1 -> issue of the group's next unit (its weight and digit waits, the hand-off and a
+    decode), cycle = mean batch + mean gap of both kinds (clocks per k-half and group)."""
+    off, batch, gap, gap_unit = [], [], [], []
+    n_batches = n_over = 0
+    t_all = t_over = 0
+    for row in rows:
+        w = [batch_windows(row, 0), batch_windows(row, 1)]
+        if not w[0] or not w[1]:
+            continue
+        t0 = w[0][0][0]
+        rel = lambda t: ((t - t0 + (1 << 31)) % (1 << 32)) - (1 << 31)      # 32-bit SM clock, relative to the first issue
+        w = [[(rel(s), rel(e)) for s, e in wg] for wg in w]
+        off += [b[0] - a[0] for a, b in zip(w[0], w[1])]
+        for g in (0, 1):
+            for i, (s, e) in enumerate(w[g]):
+                d = max(e - s, 1)
+                o = sum(max(0, min(e, e2) - max(s, s2)) for s2, e2 in w[1 - g])
+                batch.append(e - s)
+                if i + 1 < len(w[g]):
+                    (gap if i % 2 == 0 else gap_unit).append(w[g][i + 1][0] - e)
+                n_batches += 1
+                n_over += o > d / 2
+                t_all += d
+                t_over += min(o, d)
+    if not n_batches:
+        return None
+    return {"offset_clk": statistics.median(off), "overlap_batches": round(n_over / n_batches, 3),
+            "overlap_time": round(t_over / t_all, 3), "batch_clk": statistics.median(batch), "gap_clk": statistics.median(gap),
+            "unit_gap_clk": statistics.median(gap_unit) if gap_unit else None,
+            "cycle_clk": round(statistics.mean(batch) + statistics.mean(gap + gap_unit), 1) if gap + gap_unit else None}
+
+
+def unit_wait(rows):
+    """Median SM clocks a decode group spends in its per-unit wait for the unit's weights and digits (one mbarrier, W_FULL),
+    over the first four units of each group (slots 48-55: before the wait in the low word, after it in the high word)."""
+    wait = []
+    for row in rows:
+        for v in row[48:56]:
+            if v:
+                v &= (1 << 64) - 1
+                wait.append(((v >> 32) - (v & 0xffffffff)) % (1 << 32))
+    return statistics.median(wait) if wait else None
+
+
 def isolated(tok, ext, buf, reps, library):
     import torch
     results = []
@@ -48,7 +113,7 @@ def isolated(tok, ext, buf, reps, library):
             tok.run([ln])
         torch.cuda.synchronize()
         ph = {k: [] for k in ("ramp", "prologue", "digits", "steady", "tail", "total")}
-        ctas = []
+        ctas, all_rows = [], []
         ext.lib.exl3b_debug_tc_timeline(ctypes.c_void_p(buf.data_ptr()))
         try:
             for _ in range(reps):
@@ -57,6 +122,7 @@ def isolated(tok, ext, buf, reps, library):
                 torch.cuda.synchronize()
                 rows = [r for r in buf.cpu().tolist() if r[0] and r[2] and r[3] and r[4] and r[10] and r[8]]
                 ctas.append(len(rows))
+                all_rows += rows
                 for r in rows:
                     ph["ramp"].append((r[3] - r[0]) / 1e3)
                     ph["prologue"].append((r[2] - r[0]) / 1e3)
@@ -72,7 +138,8 @@ def isolated(tok, ext, buf, reps, library):
         res = {"launch": launch_name(ln), "k": mats[0]["k"], "n": [m["n"] for m in mats], "K": mats[0]["K"], "units": units,
                "ctas": n_cta, "ramp_us": q(ph["ramp"]), "prologue_us": q(ph["prologue"]), "digits_us": q(ph["digits"]),
                "steady_us": q(ph["steady"]), "tail_us": q(ph["tail"]), "cta_total_us": q(ph["total"]),
-               "steady_us_per_unit": round(statistics.median(ph["steady"]) / (units / n_cta), 3)}
+               "steady_us_per_unit": round(statistics.median(ph["steady"]) / (units / n_cta), 3),
+               "turns": turn_stats(all_rows), "unit_wait_clk": unit_wait(all_rows)}
         results.append(res)
         print(json.dumps(res), flush=True)
     return results
