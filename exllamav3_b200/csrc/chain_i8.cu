@@ -181,14 +181,17 @@ __device__ __forceinline__ void group_unit(const ChainCtx& cx, int tl, int lane,
     const int c = lane & 3;
     [[maybe_unused]] const bool tr = trace && tl == 0 && lane == 0;
     CH_STAMP(tr, 0);
-    mbar_wait<32>(cx.W_FULL(s), sph);
+    mbar_wait_ready<32>(cx.W_FULL(s), sph);
     CH_STAMP(tr, 1);
-    mbar_wait(cx.X_FULL(s), sph);                                      // the unit's activation digits
+    mbar_wait_ready(cx.X_FULL(s), sph);                                // the unit's activation digits
     CH_STAMP(tr, 2);
     const uint8_t* b = cx.smem + cx.L.off_b + s * i8_b_stage(CH_MR);
+    // the digit sum stays ahead of the MMAs here: read under k-half 0's batch, as the single-GEMM body does, it takes the
+    // chain kernel past its spill budget
     if (c < m) tsum += *reinterpret_cast<const int*>(b + i8_b_bytes(CH_MR) + 4 * c);
     I8BatchClock clk{};
-    i8_unit_mma<K, CH_MR>(reinterpret_cast<const uint32_t*>(cx.smem + s * cx.w_bytes), smem_desc(smem_u32(b), 128, 4096, 0), tl, lane, acc, clk);
+    i8_unit_mma<K, CH_MR>(reinterpret_cast<const uint32_t*>(cx.smem + s * cx.w_bytes), smem_desc(smem_u32(b), 128, 4096, 0), tl, lane, acc, clk,
+                          [] {});
     CH_STAMP(tr, 3);
     __syncwarp();
     if (lane == 0) mbar_arrive(cx.W_EMPTY(s));

@@ -351,8 +351,8 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     else if (warp >= TC_DEC_WARP0 && warp < TC_EPI_WARP0)
     {
         // =========================== decode + MMA ===========================
-        // Warpgroup (g, nh): units u = g (mod 2), output columns 64 nh .. 64 nh + 63 of the strip.  Both groups walk the same
-        // sub-segment boundaries and hand over (possibly zero) accumulators at every boundary; the epilogue adds the two.
+        // Warpgroup (g, nh): units u = g (mod 2), output columns 64 nh .. 64 nh + 63 of the strip.  A group steps through its
+        // own units only, but hands over (possibly zero) accumulators at every sub-segment boundary; the epilogue adds the two.
         const int wq = warp & 3, wgi = (warp - TC_DEC_WARP0) >> 2;
         const int g = wgi & 1, nh = wgi >> 1;
         const int tl = 4 * nh + wq;                      // tile column of the strip owned by this warp
@@ -367,53 +367,117 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
 #ifdef EXL3B_TC_DEBUG
         unsigned long long* const dbg_row = p.dbg && nh == 0 && wq == 0 && lane == 0 ? p.dbg + blockIdx.x * 64 : nullptr;
         clk.dbg = dbg_row ? dbg_row + 16 + 16 * g : nullptr;
+        // unit-gap split: row gridDim.x + blockIdx.x, seen as 128 words; words 8 + 12 (4 g + j) .. + 11 follow the group's
+        // step from its unit j < 4 to unit j + 1 (tools/i8_phase_profile.py, "unit_gap_split")
+        uint32_t* const att = dbg_row ? reinterpret_cast<uint32_t*>(p.dbg + (gridDim.x + blockIdx.x) * 64) + 8 + 48 * g : nullptr;
+        uint32_t t_ho = 0;                               // clocks in hand-offs since the group's last W_EMPTY arrival
+        int du = 0;                                      // the group's unit count
 #endif
-        int s = 0, sph = 0, dbuf = 0, dphase = 0, seg_left = 0, sub_left = 0;
-        int kb = ubeg % KB;
-        for (int u = 0; u < n_units; ++u)
+        int dbuf = 0, dphase = 0;
+        auto hand_off = [&]
         {
-            if (seg_left == 0)
-            {
-                const int to_strip_end = KB - kb;
-                seg_left = (n_units - u) < to_strip_end ? (n_units - u) : to_strip_end;
-            }
-            if (sub_left == 0) sub_left = seg_left < I8_SUB_UNITS ? seg_left : I8_SUB_UNITS;
-            if ((u & 1) == g)
-            {
 #ifdef EXL3B_TC_DEBUG
-                uint32_t t_in; asm volatile("mov.u32 %0, %%clock;" : "=r"(t_in) :: "memory");
+            const uint32_t t0 = sm_clock();
 #endif
-                mbar_wait<32>(W_FULL(s), sph);                               // the unit's weights and activation digits
-                if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) { stamp(3); stamp(4); }
-                const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
+            // hand the sub-segment's accumulators to the epilogue
+            mbar_wait(D_EMPTY(dbuf), dphase ^ 1);
+            i8_hand_off<MR>(s_d, s_dt, dbuf, g, nh, wq, lane, acc, t_lo, t_hi);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(D_FULL(dbuf));
+            dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
 #ifdef EXL3B_TC_DEBUG
-                // slots 48 + 4 g + j: SM clock before (low word) and after (high word) the wait of the group's unit j < 4
-                if (dbg_row && (u >> 1) < 4)
+            t_ho += sm_clock() - t0;
+#endif
+        };
+        auto unit = [&](int u, int s, int sph)
+        {
+#ifdef EXL3B_TC_DEBUG
+            const uint32_t t_in = sm_clock();
+            uint32_t wait_info = 0;                      // bit 31: the first probe failed; bits 0..30: ns slept after it
+            if (att)
+            {
+                // the release wait below, taken apart: mbar_wait_ready<32>
+                if (!mbar_test_wait(W_FULL(s), sph))
                 {
-                    uint32_t t_out; asm volatile("mov.u32 %0, %%clock;" : "=r"(t_out) :: "memory");
-                    dbg_row[48 + 4 * g + (u >> 1)] = ((unsigned long long) t_out << 32) | t_in;
+                    wait_info = 1u << 31;
+                    uint32_t ns = 32, polls = 0;
+                    unsigned long long t0 = 0;
+                    while (!mbar_try_wait(W_FULL(s), sph))
+                    {
+                        __nanosleep(ns); wait_info += ns; if (ns < 512u) ns <<= 1;
+                        poll_watchdog<1023u>(polls, t0, "mbarrier", (int) W_FULL(s), sph);
+                    }
                 }
+            }
+            else
 #endif
-                const int* dsum = reinterpret_cast<const int*>(smem + L.off_b + s * L.b_bytes + I8_B_BYTES);
+            mbar_wait_ready<32>(W_FULL(s), sph);                             // the unit's weights and activation digits
+#ifdef EXL3B_TC_DEBUG
+            const uint32_t t_out = sm_clock();
+#endif
+            if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) { stamp(3); stamp(4); }
+            const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
+#ifdef EXL3B_TC_DEBUG
+            // slots 48 + 4 g + j: SM clock before (low word) and after (high word) the wait of the group's unit j < 4
+            if (dbg_row && du < 4) dbg_row[48 + 4 * g + du] = ((unsigned long long) t_out << 32) | t_in;
+#endif
+            // the unit's digit sums are read and added while k-half 0's batch is in flight
+            const int* dsum = reinterpret_cast<const int*>(smem + L.off_b + s * L.b_bytes + I8_B_BYTES);
+            auto digit_sums = [&]
+            {
                 if (c < p.m) t_lo += dsum[c];
                 if (MR > 4 && c + 4 < p.m) t_hi += dsum[c + 4];
-                i8_unit_mma<K, MR>(wst, desc0 + (uint64_t) ((s * L.b_bytes) >> 4), tl, lane, acc, clk);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(W_EMPTY(s));
-                if (u == n_units - 1 && wq == 0 && lane == 0) stamp(10);
-            }
-            --seg_left; --sub_left;
-            if (sub_left == 0)
+            };
+#ifdef EXL3B_TC_DEBUG
+            const uint32_t t_dsum = sm_clock_after((uint32_t) (t_lo + t_hi));
+            if (att && du >= 1 && du <= 4)
             {
-                // hand the sub-segment's accumulators to the epilogue
-                mbar_wait(D_EMPTY(dbuf), dphase ^ 1);
-                i8_hand_off<MR>(s_d, s_dt, dbuf, g, nh, wq, lane, acc, t_lo, t_hi);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(D_FULL(dbuf));
-                dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
+                uint32_t* a = att + 12 * (du - 1);
+                a[4] = t_in; a[5] = t_out; a[6] = wait_info; a[7] = t_dsum;
             }
-            if (++kb == KB) kb = 0;
-            if (++s == S) { s = 0; sph ^= 1; }
+#endif
+            i8_unit_mma<K, MR>(wst, desc0 + (uint64_t) ((s * L.b_bytes) >> 4), tl, lane, acc, clk, digit_sums);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(W_EMPTY(s));
+            if (u == n_units - 1 && wq == 0 && lane == 0) stamp(10);
+#ifdef EXL3B_TC_DEBUG
+            if (att && du >= 1 && du <= 4)
+            {
+                uint32_t* a = att + 12 * (du - 1);
+                a[8] = clk.t_loaded0; a[9] = clk.t_issue0; a[10] = clk.t_mma0; a[11] = 1u;
+            }
+            if (att && du < 4)
+            {
+                uint32_t* a = att + 12 * du;
+                a[0] = clk.t_retired1; a[1] = clk.t_end; a[2] = sm_clock();
+            }
+            t_ho = 0;
+            ++du;
+#endif
+        };
+        // the group walks its own units only; `b` is the last unit of the current sub-segment (the epilogue's sub-segments:
+        // strip ends and every I8_SUB_UNITS units), and every boundary before the group's next unit is handed off first
+        auto sub_end = [&](int u0)
+        {
+            const int to_strip_end = KB - (ubeg + u0) % KB;
+            const int seg_end = u0 + ((n_units - u0) < to_strip_end ? (n_units - u0) : to_strip_end) - 1;
+            return seg_end < u0 + I8_SUB_UNITS - 1 ? seg_end : u0 + I8_SUB_UNITS - 1;
+        };
+        int b = sub_end(0);
+        int s = g < S ? g : g - S, sph = 0;
+        for (int u = g; ; u += 2)
+        {
+            while (b < u && b < n_units)
+            {
+                hand_off();
+                b = b + 1 < n_units ? sub_end(b + 1) : n_units;
+            }
+#ifdef EXL3B_TC_DEBUG
+            if (att && du >= 1 && du <= 4) att[12 * (du - 1) + 3] = t_ho;
+#endif
+            if (u >= n_units) break;
+            unit(u, s, sph);
+            s += 2; if (s >= S) { s -= S; sph ^= 1; }
         }
     }
     else if (warp >= TC_EPI_WARP0)

@@ -87,58 +87,99 @@ __device__ __forceinline__ void i8_write_digit_tile(uint8_t* dst, const float (&
     if (lane == 0) mbar_arrive(x_full);
 }
 
+#ifdef EXL3B_TC_DEBUG
+__device__ __forceinline__ uint32_t sm_clock()
+{
+    uint32_t t; asm volatile("mov.u32 %0, %%clock;" : "=r"(t) :: "memory"); return t;
+}
+// The SM clock once `v` is available: both predicated reads wait for the compare, so for a register loaded from shared memory
+// the stamp includes the load's latency (an unconditional read of %clock would issue right behind the load).
+__device__ __forceinline__ uint32_t sm_clock_after(uint32_t v)
+{
+    uint32_t t;
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0x9e3779b9;\n\t@p mov.u32 %0, %%clock;\n\t@!p mov.u32 %0, %%clock;\n\t}"
+                 : "=r"(t) : "r"(v) : "memory");
+    return t;
+}
+#endif
+
 // Timeline of a decode warp's k-half wgmma batches in the EXL3B_TC_DEBUG build (tools/i8_phase_profile.py): the SM clock at
-// the issue and at the retirement of each batch.  The other builds keep no state and emit nothing.
+// the issue and at the retirement of each batch, and for the unit-gap split the clock once k-half 0's weight words are in
+// registers, after its first wgmma, and after the register fences that end the unit.  The other builds keep no state and
+// emit nothing.
 struct I8BatchClock
 {
 #ifdef EXL3B_TC_DEBUG
     unsigned long long* dbg;                 // slots of the CTA's timeline row (16 batches), null: no stamps
     int i;                                   // next batch
     uint32_t t_issue;
-    __device__ __forceinline__ void issue() { asm volatile("mov.u32 %0, %%clock;" : "=r"(t_issue) :: "memory"); }
-    __device__ __forceinline__ void retired()
+    uint32_t t_loaded0, t_issue0, t_mma0;    // k-half 0: weight words loaded, fence reached (decoded), first wgmma issued
+    uint32_t t_retired1, t_end;              // k-half 1: batch retired, register fences passed
+    __device__ __forceinline__ void loaded(int r, uint32_t w) { if (r == 0) t_loaded0 = sm_clock_after(w); }
+    __device__ __forceinline__ void issue(int r) { t_issue = sm_clock(); if (r == 0) t_issue0 = t_issue; }
+    __device__ __forceinline__ void first_mma(int r) { if (r == 0) t_mma0 = sm_clock(); }
+    __device__ __forceinline__ void retired(int r)
     {
-        uint32_t t; asm volatile("mov.u32 %0, %%clock;" : "=r"(t) :: "memory");
+        const uint32_t t = sm_clock();
         if (dbg && i < 16) dbg[i] = ((unsigned long long) t << 32) | t_issue;          // retirement (high word), issue (low)
         ++i;
+        if (r == 1) t_retired1 = t;
     }
+    __device__ __forceinline__ void end() { t_end = sm_clock(); }
 #else
-    __device__ __forceinline__ void issue() {}
-    __device__ __forceinline__ void retired() {}
+    __device__ __forceinline__ void loaded(int, uint32_t) {}
+    __device__ __forceinline__ void issue(int) {}
+    __device__ __forceinline__ void first_mma(int) {}
+    __device__ __forceinline__ void retired(int) {}
+    __device__ __forceinline__ void end() {}
 #endif
 };
 
 // One unit (128 k x 128 n weights) of a decode warp: lane (chunk, c) decodes tile column `tl`, both halves, of k-tile 4 r + c
 // (r = 0, 1) from the weight stage `wst` straight into wgmma A fragments, 8 wgmma.m64nNk32 per r against the digit tile at
-// `desc_s`, into acc.  The caller has waited for both the weights and the digits.  `clk` takes the batches' issue and
-// retirement times (debug timeline).
-template <int K, int MR>
-__device__ __forceinline__ void i8_unit_mma(const uint32_t* wst, uint64_t desc_s, int tl, int lane, uint32_t (&acc)[MR], I8BatchClock& clk)
+// `desc_s`, into acc.  The caller has waited for both the weights and the digits.  `in_flight()` runs while k-half 0's batch
+// is in flight (the caller's per-unit bookkeeping; it must not touch acc).  `clk` takes the batches' issue and retirement
+// times (debug timeline).
+template <int K, int MR, typename InFlight>
+__device__ __forceinline__ void i8_unit_mma(const uint32_t* wst, uint64_t desc_s, int tl, int lane, uint32_t (&acc)[MR], I8BatchClock& clk,
+                                            InFlight&& in_flight)
 {
     const int chunk = lane >> 2, c = lane & 3;
+    // k-half 0's weight words are loaded here, k-half 1's while k-half 0's batch is in flight: its decode then starts on
+    // words already in registers (K + 1 registers next to the fragments the batch reads)
+    uint32_t w[K + 1];
+    load_chunk<K>(wst + (c * 8 + tl) * (8 * K), chunk, w);
     #pragma unroll
     for (int r = 0; r < 2; ++r)
     {
-        // the weight words of k-half r are loaded only now: one k-half's words and fragments are live at a time
-        uint32_t w[K + 1], o0[16], o1[16];
-        load_chunk<K>(wst + ((4 * r + c) * 8 + tl) * (8 * K), chunk, w);
+        uint32_t o0[16], o1[16];
+        clk.loaded(r, w[K]);
         decode16_i8<K, 0>(w, o0);
         decode16_i8<K, 1>(w, o1);
         #pragma unroll
         for (int i = 0; i < MR; ++i) reg_fence(acc[i]);
-        clk.issue();
+        clk.issue(r);
         wgmma_fence();
         #pragma unroll
         for (int j = 0; j < 8; ++j)
+        {
             wgmma_u8s8<MR>(acc, o0[2 * j], o1[2 * j], o0[2 * j + 1], o1[2 * j + 1], desc_s + (uint64_t) (16 * (8 * r + j)));
+            if (j == 0) clk.first_mma(r);
+        }
         wgmma_commit();
+        if (r == 0)
+        {
+            in_flight();
+            load_chunk<K>(wst + ((4 + c) * 8 + tl) * (8 * K), chunk, w);
+        }
         wgmma_wait<0>();
-        clk.retired();
+        clk.retired(r);
         #pragma unroll
         for (int i = 0; i < 16; ++i) { reg_fence(o0[i]); reg_fence(o1[i]); }
         #pragma unroll
         for (int i = 0; i < MR; ++i) reg_fence(acc[i]);
     }
+    clk.end();
 }
 
 // Hand a sub-segment's accumulators of decode group g to the epilogue: the registers into s_d [dbuf][g][128][2 MR], the digit

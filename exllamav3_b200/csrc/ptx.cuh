@@ -49,7 +49,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity)
                  : "=r"(ok) : "r"(bar), "r"(parity), "r"(0x989680u) : "memory");
     return ok != 0;
 }
-// non-blocking probe (diagnostics only)
+// non-blocking probe
 __device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity)
 {
     uint32_t ok;
@@ -101,6 +101,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
         if constexpr (BACKOFF_NS > 0) { __nanosleep(ns); if (ns < 16u * BACKOFF_NS) ns <<= 1; }
         poll_watchdog<1023u>(polls, t0, "mbarrier", (int) bar, (int) parity);
     }
+}
+
+// mbar_wait for a phase that has usually completed already: one non-blocking test_wait first.
+template <int BACKOFF_NS = 0>
+__device__ __forceinline__ void mbar_wait_ready(uint32_t bar, uint32_t parity)
+{
+    if (mbar_test_wait(bar, parity)) return;
+    mbar_wait<BACKOFF_NS>(bar, parity);
 }
 
 // ---- bulk async copy global -> shared (1-D), completion on an mbarrier ----------------------------------------

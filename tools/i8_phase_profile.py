@@ -21,6 +21,8 @@ of the first 16 batches of one warp per group (slots 16-47, see turn_stats): the
 batches (and of batch time) during which the other group also had a batch in flight, the batch time, the gaps between batches
 inside a unit and between units, and the cycle per k-half; unit_wait_clk is the decode group's wait for a unit's weights and
 digits (slots 48-55).  The decode warps' stamps are SM clocks: one clock per SM, compared only inside a CTA.
+"unit_gap_split" takes a group's step between units apart (a second timeline row per CTA, see unit_gap_split).  The stamps'
+own global stores lie on that path, so the timeline build's steps are longer than the production kernel's.
 
 --replay: what a launch costs between its predecessor and its first MMA inside the token, where PDL lets a launch start
 before the previous one ends.  Captures two layers' launches and the lm_head into one CUDA graph exactly as bench.py issues
@@ -103,6 +105,68 @@ def unit_wait(rows):
     return statistics.median(wait) if wait else None
 
 
+SPLIT_SEGMENTS = ("fences", "arrive", "handoff", "step", "wait", "digit_sums", "lds", "decode", "fence_to_mma", "total")
+
+
+def words32(row):
+    """A timeline row (64 signed u64 slots) as 128 u32 words, low word first."""
+    out = []
+    for v in row:
+        v &= (1 << 64) - 1
+        out += [v & 0xffffffff, v >> 32]
+    return out
+
+
+def unit_gap_split(att_rows):
+    """A decode group's step from k-half 1 of its unit j retired to the first wgmma of unit j + 1, split into segments
+    (SM clocks of one warp per group, the first four steps of each group; words 8 + 12 (4 g + j) of the second timeline
+    row of each CTA, see gemm_tc_i8_body.cuh):
+        fences        wgmma_wait<0> retired -> the register fences at the end of i8_unit_mma passed
+        arrive        __syncwarp and the W_EMPTY arrival
+        handoff       accumulator hand-offs in the step (D_EMPTY wait included), 0 for most steps
+        step          the rest of the loop step up to the W_FULL wait (hand-offs excluded)
+        wait          the W_FULL wait; split into wait_ready (the first probe found the phase complete) and wait_backoff
+                      (the try_wait loop ran; sleep_ns is the nanosleep time in it)
+        digit_sums    wait -> the digit sums in a register (the digit-sum LDS and add where they come before the MMAs)
+        lds           load_chunk, until the K + 1 weight words are in registers
+        decode        decode16_i8 of k-half 0
+        fence_to_mma  wgmma_fence -> the first wgmma issued
+    Per segment the median and the mean (the means add up to the mean total)."""
+    seg = {k: [] for k in SPLIT_SEGMENTS}
+    ready, backoff, sleep_ns = [], [], []
+    d = lambda a, b: (b - a) % (1 << 32)
+    for row in att_rows:
+        w = words32(row)
+        for gj in range(8):
+            a = w[8 + 12 * gj: 20 + 12 * gj]
+            if a[11] != 1:
+                continue
+            t_ret, t_end, t_arr, t_ho, t_in, t_out, info, t_dsum, t_ld, t_iss, t_mma, _ = a
+            seg["fences"].append(d(t_ret, t_end))
+            seg["arrive"].append(d(t_end, t_arr))
+            seg["handoff"].append(t_ho)
+            seg["step"].append(d(t_arr, t_in) - t_ho)
+            wt = d(t_in, t_out)
+            seg["wait"].append(wt)
+            (backoff if info >> 31 else ready).append(wt)
+            if info >> 31:
+                sleep_ns.append(info & 0x7fffffff)
+            seg["digit_sums"].append(d(t_out, t_dsum))
+            seg["lds"].append(d(t_dsum, t_ld))
+            seg["decode"].append(d(t_ld, t_iss))
+            seg["fence_to_mma"].append(d(t_iss, t_mma))
+            seg["total"].append(d(t_ret, t_mma))
+    if not seg["total"]:
+        return None
+    out = {k: {"median": statistics.median(v), "mean": round(statistics.mean(v), 1)} for k, v in seg.items()}
+    n = len(seg["total"])
+    out["wait_ready"] = {"share": round(len(ready) / n, 3), "median": statistics.median(ready) if ready else None}
+    out["wait_backoff"] = {"share": round(len(backoff) / n, 3), "median": statistics.median(backoff) if backoff else None,
+                           "sleep_ns_median": statistics.median(sleep_ns) if sleep_ns else None}
+    out["steps"] = n
+    return out
+
+
 def isolated(tok, ext, buf, reps, library):
     import torch
     results = []
@@ -113,14 +177,17 @@ def isolated(tok, ext, buf, reps, library):
             tok.run([ln])
         torch.cuda.synchronize()
         ph = {k: [] for k in ("ramp", "prologue", "digits", "steady", "tail", "total")}
-        ctas, all_rows = [], []
+        ctas, all_rows, att_rows = [], [], []
         ext.lib.exl3b_debug_tc_timeline(ctypes.c_void_p(buf.data_ptr()))
         try:
             for _ in range(reps):
                 buf.zero_()
                 tok.run([ln])
                 torch.cuda.synchronize()
-                rows = [r for r in buf.cpu().tolist() if r[0] and r[2] and r[3] and r[4] and r[10] and r[8]]
+                full = buf.cpu().tolist()
+                grid = sum(1 for r in full if r[0])          # every CTA stamps slot 0; rows grid .. 2 grid - 1: unit-gap split
+                att_rows += full[grid: 2 * grid]
+                rows = [r for r in full if r[0] and r[2] and r[3] and r[4] and r[10] and r[8]]
                 ctas.append(len(rows))
                 all_rows += rows
                 for r in rows:
@@ -139,7 +206,7 @@ def isolated(tok, ext, buf, reps, library):
                "ctas": n_cta, "ramp_us": q(ph["ramp"]), "prologue_us": q(ph["prologue"]), "digits_us": q(ph["digits"]),
                "steady_us": q(ph["steady"]), "tail_us": q(ph["tail"]), "cta_total_us": q(ph["total"]),
                "steady_us_per_unit": round(statistics.median(ph["steady"]) / (units / n_cta), 3),
-               "turns": turn_stats(all_rows), "unit_wait_clk": unit_wait(all_rows)}
+               "turns": turn_stats(all_rows), "unit_wait_clk": unit_wait(all_rows), "unit_gap_split": unit_gap_split(att_rows)}
         results.append(res)
         print(json.dumps(res), flush=True)
     return results
