@@ -12,8 +12,9 @@
 //     a global counter, and only the warps that PREPARE activations wait for it.  The TMA producer and the decode warps
 //     run on into the next stage's weights (they depend on no activation), so HBM streams through the boundary and the
 //     first operand stages of the next GEMM are decoded before its input exists.
-//   * the unit pipeline itself is the one of gemm_tc_i8_body.cuh (two decode groups of two warpgroups, each warpgroup
-//     decoding its weights straight into wgmma A fragments and accumulating in registers).
+//   * the unit pipeline itself is the one of gemm_tc_i8_body.cuh (i8_pipeline.cuh: two decode groups of two warpgroups,
+//     each warpgroup decoding its weights straight into wgmma A fragments and accumulating in registers; the same ring
+//     barriers, one W_FULL wait per unit for its weights and digits, the same row transform and split-K exchange).
 //   * activation scale without a Hadamard pass.  The quantisation scale only needs an upper bound of max |xh| over
 //     the row; xh is a block-orthonormal transform of x * suh, so max_kb || (x * suh)_kb ||_2 is one -- a plain
 //     reduction pass over the row by three warps (which also applies silu * mul for the gated-MLP input and caches
@@ -62,7 +63,6 @@ struct ChainParams
     int S, w_bytes, cache_bytes, suh_bytes;
     unsigned int* ctr;        // [n_stages] finished output segments per stage, [n_stages] exit ticket; zero between launches
     float* parts;             // split-K exchange, [2][grid][MR * 128] words, sentinel between launches
-    unsigned long long* dbg;
     ChainOp ops_inline[CH_MAX_INLINE];
     ChainStage stages_inline[CH_MAX_INLINE];
     CUtensorMap tmaps_inline[CH_MAX_INLINE];
@@ -153,38 +153,21 @@ __device__ __forceinline__ float silu_f32(float x) { return x * __fdividef(1.0f,
 struct ChainCtx
 {
     uint8_t* smem;
-    uint32_t bar0;
-    int S, w_bytes;
+    I8Bars bars;
+    int w_bytes;
     ChainSmem L;
-    unsigned long long* dbg;
-    int trace_seq;            // bring-up: the unit (CTA-local index) whose steps are stamped
-    __device__ __forceinline__ uint32_t W_FULL(int s) const { return bar0 + 8u * s; }
-    __device__ __forceinline__ uint32_t W_EMPTY(int s) const { return bar0 + 8u * (TC_MAX_STAGES + s); }
-    __device__ __forceinline__ uint32_t X_FULL(int s) const { return bar0 + 8u * (2 * TC_MAX_STAGES + s); }
-    __device__ __forceinline__ uint32_t D_FULL(int b) const { return bar0 + 8u * (3 * TC_MAX_STAGES + 8 + b); }
-    __device__ __forceinline__ uint32_t D_EMPTY(int b) const { return bar0 + 8u * (3 * TC_MAX_STAGES + 10 + b); }
-    __device__ __forceinline__ uint32_t IN_BAR() const { return bar0 + 8u * (3 * TC_MAX_STAGES + 12); }
+    // after the ring's barriers: the op's suh copy and its input rows (bulk copies or plain arrivals)
+    __device__ __forceinline__ uint32_t IN_BAR() const { return bars.end(); }
 };
-constexpr int CH_NUM_BARS = 3 * TC_MAX_STAGES + 13;                    // 61 barriers
+// the chain lays the ring's barrier block out for the deepest ring; IN_BAR follows it, then the misc words
+constexpr int CH_NUM_BARS = I8Bars::words(TC_MAX_STAGES) + 1;
 
-#ifdef EXL3B_TC_DEBUG
-#define CH_STAMP(cond, slot) do { if ((cond) && cx.dbg) { unsigned long long t__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t__) :: "memory"); cx.dbg[blockIdx.x * 64 + (slot)] = t__; } } while (0)
-#else
-#define CH_STAMP(cond, slot) do { } while (0)
-#endif
-
-// One unit of a decode warp: wait for the ring stage's weights and digits, then i8_unit_mma.
+// One unit of a decode warp: wait for the ring stage's weights and digits (W_FULL), then i8_unit_mma.
 template <int K>
-__device__ __forceinline__ void group_unit(const ChainCtx& cx, int tl, int lane, int s, int sph, int m, uint32_t (&acc)[CH_MR], int& tsum,
-                                           [[maybe_unused]] bool trace)
+__device__ __forceinline__ void group_unit(const ChainCtx& cx, int tl, int lane, int s, int sph, int m, uint32_t (&acc)[CH_MR], int& tsum)
 {
     const int c = lane & 3;
-    [[maybe_unused]] const bool tr = trace && tl == 0 && lane == 0;
-    CH_STAMP(tr, 0);
-    mbar_wait_ready<32>(cx.W_FULL(s), sph);
-    CH_STAMP(tr, 1);
-    mbar_wait_ready(cx.X_FULL(s), sph);                                // the unit's activation digits
-    CH_STAMP(tr, 2);
+    mbar_wait_ready<32>(cx.bars.W_FULL(s), sph);
     const uint8_t* b = cx.smem + cx.L.off_b + s * i8_b_stage(CH_MR);
     // the digit sum stays ahead of the MMAs here: read under k-half 0's batch, as the single-GEMM body does, it takes the
     // chain kernel past its spill budget
@@ -192,9 +175,8 @@ __device__ __forceinline__ void group_unit(const ChainCtx& cx, int tl, int lane,
     I8BatchClock clk{};
     i8_unit_mma<K, CH_MR>(reinterpret_cast<const uint32_t*>(cx.smem + s * cx.w_bytes), smem_desc(smem_u32(b), 128, 4096, 0), tl, lane, acc, clk,
                           [] {});
-    CH_STAMP(tr, 3);
     __syncwarp();
-    if (lane == 0) mbar_arrive(cx.W_EMPTY(s));
+    if (lane == 0) mbar_arrive(cx.bars.W_EMPTY(s));
 }
 
 // KSEL = 0: ops of any bitrate (a switch per unit); KSEL = 1..8: every op of the chain has K = KSEL (smaller code: the
@@ -210,11 +192,8 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
     const CUtensorMap* tmaps = p.n_inline ? p.tmaps_inline : p.tmaps;
     const int S = p.S;
     ChainCtx cx;
-    cx.smem = smem; cx.S = S; cx.w_bytes = p.w_bytes; cx.L = chain_smem(S, p.w_bytes, p.cache_bytes, p.suh_bytes);
-    cx.dbg = p.dbg; cx.trace_seq = 8;
-    CH_STAMP(threadIdx.x == 0, 61);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + cx.L.off_bars);
-    cx.bar0 = smem_u32(bars);
+    cx.smem = smem; cx.w_bytes = p.w_bytes; cx.L = chain_smem(S, p.w_bytes, p.cache_bytes, p.suh_bytes);
+    cx.bars = I8Bars{smem_u32(smem + cx.L.off_bars), TC_MAX_STAGES};
     uint32_t* misc = reinterpret_cast<uint32_t*>(smem + cx.L.off_bars + 8 * CH_NUM_BARS);
     unsigned int* s_norm2 = reinterpret_cast<unsigned int*>(misc + 4);                                       // [MR] float bits
     float* s_scale = reinterpret_cast<float*>(misc + 8 + 8);                                                 // [CH_SCALE_SLOTS][MR]
@@ -229,11 +208,12 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
         for (int i = lane; i < CH_NUM_BARS; i += 32)
         {
             int cnt = 1;
-            if (i >= TC_MAX_STAGES && i < 2 * TC_MAX_STAGES) cnt = TC_DEC_WARPS / I8_DEC_GROUPS;         // W_EMPTY: the group's warps, after their MMAs
-            else if (i >= 3 * TC_MAX_STAGES + 8 && i < 3 * TC_MAX_STAGES + 10) cnt = TC_DEC_WARPS;         // D_FULL: every decode warp
-            else if (i >= 3 * TC_MAX_STAGES + 10 && i < 3 * TC_MAX_STAGES + 12) cnt = 4;                 // D_EMPTY: the 4 epilogue warps
-            else if (i == 3 * TC_MAX_STAGES + 12) cnt = 2;                                               // IN_BAR: suh copy + input copy
-            mbar_init(cx.bar0 + 8u * i, cnt);
+            if (i < TC_MAX_STAGES) cnt = I8Bars::W_FULL_ARRIVALS;
+            else if (i < 2 * TC_MAX_STAGES) cnt = I8Bars::W_EMPTY_ARRIVALS;
+            else if (i >= 3 * TC_MAX_STAGES + 8 && i < 3 * TC_MAX_STAGES + 10) cnt = I8Bars::D_FULL_ARRIVALS;
+            else if (i >= 3 * TC_MAX_STAGES + 10 && i < 3 * TC_MAX_STAGES + 12) cnt = I8Bars::D_EMPTY_ARRIVALS;
+            else if (i == I8Bars::words(TC_MAX_STAGES)) cnt = 2;                                         // IN_BAR: suh copy + input copy
+            mbar_init(cx.bars.bar0 + 8u * i, cnt);
         }
         fence_barrier_init();
     }
@@ -257,11 +237,11 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                 tm = tmaps + cur_op;
                 if (elect_one()) prefetch_tmap(tm);
             }
-            mbar_wait<64>(cx.W_EMPTY(s), ph ^ 1);
+            mbar_wait<64>(cx.bars.W_EMPTY(s), ph ^ 1);
             if (elect_one())
             {
-                mbar_arrive_expect_tx(cx.W_FULL(s), (uint32_t) (2048 * K));
-                tma_load_2d(w_smem0 + s * p.w_bytes, tm, c.strip * (32 * K), c.kb * 8, cx.W_FULL(s), pol_w);
+                mbar_arrive_expect_tx(cx.bars.W_FULL(s), (uint32_t) (2048 * K));
+                tma_load_2d(w_smem0 + s * p.w_bytes, tm, c.strip * (32 * K), c.kb * 8, cx.bars.W_FULL(s), pol_w);
             }
             if (++s == S) { s = 0; ph ^= 1; }
             c.next();
@@ -292,7 +272,6 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                     o.A = g.A; o.A2 = g.A2; o.suh = g.suh; o.m = g.m; o.k = g.k; o.KB = g.KB; o.in_mode = g.in_mode;
                     o.cached = g.cached; o.suh_cached = g.suh_cached; o.stage = g.stage;
                 }
-                CH_STAMP(warp == TC_XF_WARP0 && lane == 0 && c.seq == 0, 59);
                 const bool bulk_x = o.in_mode == 0 && o.cached;       // input rows by one bulk copy straight into the cache
                 const bool bulk_s = o.suh != nullptr && o.suh_cached;
                 xf_bar();                                             // previous op's cache / suh no longer needed by any digit warp
@@ -425,49 +404,37 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
                     const float n2 = __uint_as_float(s_norm2[r]);
                     const float bnd = (n2 > 0.f ? i8_sqrt_rn(n2) : 0.f) * 1.002f;   // n2: 0 or in [2^-48, 2^40]
                     inv_scale[r] = bnd > 0.f ? i8_qmax_over(bnd) : 0.f;
-                    // every digit warp stores the (identical) value before its own first X_FULL arrive of this op: whichever
-                    // arrive the MMA side observes, the scale the epilogue reads later is ordered before it
+                    // every digit warp stores the (identical) value before its own first W_FULL arrival of this op: whichever
+                    // arrival the MMA side observes, the scale the epilogue reads later is ordered before it
                     if (lane == r) s_scale[(cur_op % CH_SCALE_SLOTS) * CH_MR + r] = i8_over_qmax(bnd);
                 }
-                CH_STAMP(warp == TC_XF_WARP0 && lane == 0 && c.seq == 0, 60);
             }
             if (turn == xw)
             {
                 // ---- digits of this unit: 128-point Hadamard of the cached block, quantise, two int8 digits x 4 bytes ----
-                CH_STAMP(c.seq == cx.trace_seq && lane == 0, 56);
-                mbar_wait<64>(cx.W_EMPTY(s), ph ^ 1);
-                CH_STAMP(c.seq == cx.trace_seq && lane == 0, 57);
-                i8_write_digit_tile<CH_MR>(smem + cx.L.off_b + s * i8_b_stage(CH_MR), inv_scale, o.m, lane, cx.X_FULL(s),
+                mbar_wait<64>(cx.bars.W_EMPTY(s), ph ^ 1);
+                i8_write_digit_tile<CH_MR>(smem + cx.L.off_b + s * i8_b_stage(CH_MR), inv_scale, o.m, lane, cx.bars.W_FULL(s),
                                            [&](int r, float (&v)[4])
                 {
-                    half2 a, b;
-                    if (o.cached)
-                    {
-                        const uint2 raw = *reinterpret_cast<const uint2*>(cache + (size_t) r * o.k + c.kb * 128 + lane * 4);
-                        a = *reinterpret_cast<const half2*>(&raw.x); b = *reinterpret_cast<const half2*>(&raw.y);
-                    }
+                    uint2 raw;
+                    if (o.cached) raw = *reinterpret_cast<const uint2*>(cache + (size_t) r * o.k + c.kb * 128 + lane * 4);
                     else
                     {
-                        // rows too long for the cache: recompute the block (plain fp16 input only, checked on the host)
-                        const uint2 raw = __ldcg(reinterpret_cast<const uint2*>(reinterpret_cast<const half*>(o.A) + (size_t) r * o.k + c.kb * 128 + lane * 4));
-                        a = *reinterpret_cast<const half2*>(&raw.x); b = *reinterpret_cast<const half2*>(&raw.y);
+                        // rows too long for the cache: recompute x * suh (plain fp16 input only, checked on the host)
+                        raw = __ldcg(reinterpret_cast<const uint2*>(reinterpret_cast<const half*>(o.A) + (size_t) r * o.k + c.kb * 128 + lane * 4));
                         if (o.suh)
                         {
                             const uint2 scb = *reinterpret_cast<const uint2*>(o.suh + c.kb * 128 + lane * 4);
-                            a = __hmul2(a, *reinterpret_cast<const half2*>(&scb.x));
-                            b = __hmul2(b, *reinterpret_cast<const half2*>(&scb.y));
+                            half2* h = reinterpret_cast<half2*>(&raw);
+                            h[0] = __hmul2(h[0], *reinterpret_cast<const half2*>(&scb.x));
+                            h[1] = __hmul2(h[1], *reinterpret_cast<const half2*>(&scb.y));
                         }
                     }
-                    if (o.suh)
-                    {
-                        float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
-                        had128_warp(v0, v1, v2, v3, lane);
-                        a = __floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE);
-                        b = __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE);
-                    }
+                    // one Hadamard for both: x * suh is already applied (the cache holds it)
+                    if (o.suh) raw = had128_fp16(raw, nullptr, lane);
+                    const half2 a = *reinterpret_cast<const half2*>(&raw.x), b = *reinterpret_cast<const half2*>(&raw.y);
                     v[0] = __low2float(a); v[1] = __high2float(a); v[2] = __low2float(b); v[3] = __high2float(b);
                 });
-                CH_STAMP(c.seq == cx.trace_seq && lane == 0, 58);
             }
             if (++turn == CH_XF_WARPS) turn = 0;
             if (++s == S) { s = 0; ph ^= 1; }
@@ -491,17 +458,16 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
             const bool last = c.seq == se - 1;
             if ((c.seq & 1) == g)
             {
-                const bool trace = c.seq == cx.trace_seq;
                 const int m = ops[c.op].m;
-                if constexpr (KSEL != 0) group_unit<KSEL>(cx, tl, lane, s, ph, m, acc, tsum, trace);
-                else EXL3B_DISPATCH_K(ops[c.op].K, group_unit<KK>(cx, tl, lane, s, ph, m, acc, tsum, trace));
+                if constexpr (KSEL != 0) group_unit<KSEL>(cx, tl, lane, s, ph, m, acc, tsum);
+                else EXL3B_DISPATCH_K(ops[c.op].K, group_unit<KK>(cx, tl, lane, s, ph, m, acc, tsum));
             }
             if (last)
             {
-                mbar_wait(cx.D_EMPTY(dbuf), dphase ^ 1);               // the epilogue has drained this buffer
+                mbar_wait(cx.bars.D_EMPTY(dbuf), dphase ^ 1);          // the epilogue has drained this buffer
                 i8_hand_off<CH_MR>(s_d, s_dt, dbuf, g, nh, wq, lane, acc, tsum, t_hi);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(cx.D_FULL(dbuf));
+                if (lane == 0) mbar_arrive(cx.bars.D_FULL(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
             }
             if (++s == S) { s = 0; ph ^= 1; }
@@ -538,10 +504,10 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
             for (int r = 0; r < CH_MR; ++r) facc[r] = 0.f;
             for (int sb = run_begin; sb < run_end; sb += I8_SUB_UNITS)
             {
-                mbar_wait<32>(cx.D_FULL(dbuf), dphase);
+                mbar_wait<32>(cx.bars.D_FULL(dbuf), dphase);
                 i8_drain<CH_MR>(s_d, s_dt, dbuf, col, o.m, [&](int r) { return s_scale[(op % CH_SCALE_SLOTS) * CH_MR + r]; }, facc);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(cx.D_EMPTY(dbuf));
+                if (lane == 0) mbar_arrive(cx.bars.D_EMPTY(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
             }
 
@@ -576,7 +542,6 @@ chain_i8_kernel(const __grid_constant__ ChainParams p)
     }
 
     __syncthreads();
-    CH_STAMP(threadIdx.x == 0, 62);
     if (threadIdx.x == 0)
     {
         // last CTA out re-zeroes the counters for the next launch (which reads them only after griddepcontrol.wait)
@@ -755,7 +720,6 @@ int chain_run(cudaStream_t stream, void* chain)
     EXL3B_CHECK(ch, EXL3B_ERR_ARG, "exl3_chain_run: null chain");
     int dev = -1; EXL3B_CUDA(cudaGetDevice(&dev));
     EXL3B_CHECK(dev == ch->device, EXL3B_ERR_ARG, "exl3_chain_run: chain was created on device %d, current device is %d", ch->device, dev);
-    ch->p.dbg = g_tc_dbg;
     cudaError_t err = chain_launch(stream, ch->grid, ch->smem_total, ch->p, ch->ksel);
     count_launch();
     EXL3B_CUDA(err);
@@ -789,7 +753,7 @@ int launch_gemm_chain(cudaStream_t stream, DevCtx* ctx, const GemmArgs& a)
     ChainParams& p = ch.p;
     { int r = get_weight_tmap(a.B, a.k, a.n, a.K, &p.tmaps_inline[0]); if (r) return r; }
     p.ops_inline[0] = ch.ops[0]; p.stages_inline[0] = ch.stages[0];
-    p.n_inline = 1; p.ctr = ctx->chain_ctr; p.parts = ctx->chain_parts; p.dbg = g_tc_dbg;
+    p.n_inline = 1; p.ctr = ctx->chain_ctr; p.parts = ctx->chain_parts;
     cudaError_t err = chain_launch(stream, ch.grid, ch.smem_total, p, ch.ksel);
     count_launch();
     EXL3B_CUDA(err);

@@ -292,6 +292,25 @@ __device__ __forceinline__ void had128_warp_tail(float& h0, float& h1, float& h2
     }
 }
 
+// The input transform of lane's four values k = 4 lane .. 4 lane + 3 of one 128-k block (fp16 pairs in `raw`, one block per
+// warp), as the reference's A_had: x * suh in fp16 (`scb`: lane's four suh scales; null when x already carries them), the
+// 128-point Hadamard in fp32, then * 1/sqrt(128) rounded once to fp16.  Returns the two fp16 pairs.
+__device__ __forceinline__ uint2 had128_fp16(uint2 raw, const uint2* scb, int lane)
+{
+    half2 a = *reinterpret_cast<half2*>(&raw.x), b = *reinterpret_cast<half2*>(&raw.y);
+    if (scb)
+    {
+        a = __hmul2(a, *reinterpret_cast<const half2*>(&scb->x));
+        b = __hmul2(b, *reinterpret_cast<const half2*>(&scb->y));
+    }
+    float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
+    had128_warp(v0, v1, v2, v3, lane);
+    a = __floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE);
+    b = __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE);
+    uint2 o; o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
+    return o;
+}
+
 __device__ __forceinline__ uint32_t pack_half2(half a, half b)
 {
     return (uint32_t) __half_as_ushort(a) | ((uint32_t) __half_as_ushort(b) << 16);

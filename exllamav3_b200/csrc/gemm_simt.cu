@@ -251,16 +251,9 @@ mgemm_had_kernel(const half* __restrict__ A, half* __restrict__ A_had, const uin
     const half* suh = (const half*) suh_ptrs[mat];
     const half* src = (bszm_in == 1 ? A : A + (size_t) z * m * k) + (size_t) warp * 128 + lane * 4;
     half* dst = A_had + (size_t) z * m * k + (size_t) warp * 128 + lane * 4;
-    uint2 raw = *reinterpret_cast<const uint2*>(src);
-    uint2 scb = *reinterpret_cast<const uint2*>(suh + (warp % bpr) * 128 + lane * 4);
-    half2 a = __hmul2(*reinterpret_cast<half2*>(&raw.x), *reinterpret_cast<half2*>(&scb.x));
-    half2 b = __hmul2(*reinterpret_cast<half2*>(&raw.y), *reinterpret_cast<half2*>(&scb.y));
-    float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
-    had128_warp(v0, v1, v2, v3, lane);
-    a = __floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE);
-    b = __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE);
-    uint2 o; o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
-    *reinterpret_cast<uint2*>(dst) = o;
+    const uint2 raw = *reinterpret_cast<const uint2*>(src);
+    const uint2 scb = *reinterpret_cast<const uint2*>(suh + (warp % bpr) * 128 + lane * 4);
+    *reinterpret_cast<uint2*>(dst) = had128_fp16(raw, &scb, lane);
 }
 
 // Weighted-MoE reduction: groups of (n_active / num_tokens) slots are summed into C[t] in C's dtype

@@ -84,15 +84,7 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
     auto X_FULL = [&](int s) { return bar0 + 8u * (2 * S + s); };
     int* s_flag = reinterpret_cast<int*>(smem + L.off_bars + 8 * (3 * TC_MAX_STAGES + 20));
 
-    auto stamp = [&](int slot)
-    {
-#ifdef EXL3B_TC_DEBUG
-        if (p.dbg) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); p.dbg[blockIdx.x * 64 + slot] = t; }
-#else
-        (void) slot;
-#endif
-    };
-    if (threadIdx.x == 0) stamp(0);
+    if (threadIdx.x == 0) tc_stamp(p.dbg, 0);
     pdl_launch_dependents();
 
     if (warp == 0)
@@ -102,7 +94,7 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
         fence_barrier_init();
     }
     __syncthreads();
-    if (threadIdx.x == 0) stamp(1);
+    if (threadIdx.x == 0) tc_stamp(p.dbg, 1);
 
     // ---- this CTA's unit range ----
     const int KB = p.k / 128;
@@ -144,7 +136,7 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
         for (int u = 0; u < pre; ++u) { issue_w(u, strip, kb); next_unit(); }   // weights never depend on the previous kernel
         pdl_wait();                                                              // activations do
         { int kbx = kb0; for (int u = 0; u < pre; ++u) { issue_x(u, kbx); if (++kbx == KB) kbx = 0; } }
-        if (lane == 0) stamp(2);
+        if (lane == 0) tc_stamp(p.dbg, 2);
         int s = (pre == S) ? 0 : pre, ph = (pre == S) ? 1 : 0;                   // ring position of unit `pre`
         for (int u = pre; u < n_units; ++u)
         {
@@ -202,7 +194,7 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
             for (int i = 0; i < seg; ++i)
             {
                 mbar_wait<32>(W_FULL(s), sph);
-                if (u + i == 0 && ct == 0) stamp(3);
+                if (u + i == 0 && ct == 0) tc_stamp(p.dbg, 3);
                 uint32_t w[2][K + 1];
                 f16_load_unit<K>(reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes), tl, chunk, c, w);
                 mbar_wait(X_FULL(s), sph);
@@ -245,7 +237,7 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
             cons_bar();                                              // the previous segment's readers of the tile are done
             f16_store_tile(tile, acc, tl, chunk, c, nchunks);
             f16_zero(acc);
-            if (u + seg >= n_units && ct == 0) stamp(7);
+            if (u + seg >= n_units && ct == 0) tc_stamp(p.dbg, 7);
             if (full) emit_rows(strip);
             else
             {
@@ -276,12 +268,12 @@ gemm_tc_kernel(const TcParams p, const __grid_constant__ CUtensorMap tmap_w)
             }
             u += seg;
         }
-        if (ct == 0) stamp(8);
+        if (ct == 0) tc_stamp(p.dbg, 8);
     }
 
     // ---- teardown ----
     __syncthreads();
-    if (threadIdx.x == 0) stamp(9);
+    if (threadIdx.x == 0) tc_stamp(p.dbg, 9);
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------

@@ -128,26 +128,11 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         else tmap_patch_address(smem_u32(stm), gtm, p.B_ptrs[mat], lane);
     }
 
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
-    const uint32_t bar0 = smem_u32(bars);
-    // W_FULL(s): the unit's weights (TMA bytes) AND its activation digits (the digit warp's arrival), so that a decode warp
-    // takes one barrier per unit
-    auto W_FULL = [&](int s) { return bar0 + 8u * s; };
-    auto W_EMPTY = [&](int s) { return bar0 + 8u * (S + s); };
-    auto D_FULL = [&](int s) { return bar0 + 8u * (3 * S + 8 + s); };
-    auto D_EMPTY = [&](int s) { return bar0 + 8u * (3 * S + 10 + s); };
+    const I8Bars bars{smem_u32(smem + L.off_bars), S};
     uint32_t* misc = reinterpret_cast<uint32_t*>(smem + L.off_bars + 8 * (3 * TC_MAX_STAGES + 16));
     unsigned int* s_absmax = reinterpret_cast<unsigned int*>(misc + 4);           // [MR] float bits, >= 0
     [[maybe_unused]] volatile unsigned int* s_ar = reinterpret_cast<volatile unsigned int*>(misc + 28);   // AR: epoch of this launch
 
-    auto stamp = [&](int slot)
-    {
-#ifdef EXL3B_TC_DEBUG
-        if (p.dbg) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory"); p.dbg[blockIdx.x * 64 + slot] = t; }
-#else
-        (void) slot;
-#endif
-    };
 #ifdef EXL3B_TC_DEBUG
     // how often did a role find its barrier not yet complete (= it had to wait)?  slots 56.. of the CTA's debug row
     int wf_a = 0, wf_b = 0, wf_c = 0;
@@ -155,21 +140,12 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
 #else
 #define I8_WAITCNT(cnt, bar, par) do { } while (0)
 #endif
-    if (threadIdx.x == 0) stamp(0);
+    if (threadIdx.x == 0) tc_stamp(p.dbg, 0);
     pdl_launch_dependents();
 
-    if (warp == 0)
-    {
-        // one barrier per lane and round instead of ~60 serial initialisations by one thread
-        // W_FULL: the producer (expect_tx) and the unit's digit warp; W_EMPTY: the eight decode warps of the unit's group, after
-        // their MMAs have read the weights and the digit tile
-        for (int s = lane; s < S; s += 32) { mbar_init(W_FULL(s), 2); mbar_init(W_EMPTY(s), TC_DEC_WARPS / I8_DEC_GROUPS); }
-        if (lane < 2) { mbar_init(D_FULL(lane), TC_DEC_WARPS); mbar_init(D_EMPTY(lane), 4); }
-        else if (lane < 2 + MR) s_absmax[lane - 2] = 0u;
-        fence_barrier_init();
-    }
+    if (warp == 0) bars.init(lane, [&] { if (lane < 2 + MR) s_absmax[lane - 2] = 0u; });
     __syncthreads();
-    if (threadIdx.x == 0) stamp(1);
+    if (threadIdx.x == 0) tc_stamp(p.dbg, 1);
 
     const int KB = p.k / 128;
     const int strips = n_loc / 128;
@@ -188,16 +164,8 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
     // fp16 transformed activation of (row r, k-block kb), 4 values per lane, exactly as the reference's A_had
     auto xh_finish = [&](uint2 raw, uint2 scb, float (&v)[4])
     {
-        half2 a = *reinterpret_cast<half2*>(&raw.x), b = *reinterpret_cast<half2*>(&raw.y);
-        if (suh)
-        {
-            a = __hmul2(a, *reinterpret_cast<const half2*>(&scb.x));
-            b = __hmul2(b, *reinterpret_cast<const half2*>(&scb.y));
-            float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
-            had128_warp(v0, v1, v2, v3, lane);
-            a = __floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE);
-            b = __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE);
-        }
+        if (suh) raw = had128_fp16(raw, &scb, lane);
+        const half2 a = *reinterpret_cast<half2*>(&raw.x), b = *reinterpret_cast<half2*>(&raw.y);
         v[0] = __low2float(a); v[1] = __high2float(a); v[2] = __low2float(b); v[3] = __high2float(b);
     };
     auto xh_block = [&](int r, int kb, float (&v)[4])
@@ -284,7 +252,7 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         if (p.m == 1) transform(std::integral_constant<int, 1>());
         else transform(std::integral_constant<int, MR>());
         asm volatile("bar.sync 2, %0;" :: "n"(TC_THREADS - 32) : "memory");
-        if (warp == TC_DEC_WARP0 && lane == 0) stamp(2);
+        if (warp == TC_DEC_WARP0 && lane == 0) tc_stamp(p.dbg, 2);
     }
 
     if (warp == 0)
@@ -299,11 +267,11 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         int s = 0, ph = 0;
         for (int u = 0; u < n_units; ++u)
         {
-            if (u >= S) { I8_WAITCNT(wf_a, W_EMPTY(s), ph ^ 1); mbar_wait<64>(W_EMPTY(s), ph ^ 1); }
+            if (u >= S) { I8_WAITCNT(wf_a, bars.W_EMPTY(s), ph ^ 1); mbar_wait<64>(bars.W_EMPTY(s), ph ^ 1); }
             if (elect_one())
             {
-                mbar_arrive_expect_tx(W_FULL(s), (uint32_t) L.w_bytes);
-                tma_load_2d(w_smem0 + s * L.w_bytes, tm, strip * (32 * K), kb * 8, W_FULL(s), pol_w);
+                mbar_arrive_expect_tx(bars.W_FULL(s), (uint32_t) L.w_bytes);
+                tma_load_2d(w_smem0 + s * L.w_bytes, tm, strip * (32 * K), kb * 8, bars.W_FULL(s), pol_w);
             }
             if (++kb == KB) { kb = 0; ++strip; }
             if (++s == S) { s = 0; ph ^= 1; }
@@ -329,9 +297,9 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
         const int kstep = 2 % KB;
         for (int u = xw; u < n_units; u += 2)
         {
-            I8_WAITCNT(wf_a, W_EMPTY(s), ph ^ 1);
-            mbar_wait<64>(W_EMPTY(s), ph ^ 1);
-            i8_write_digit_tile<MR>(smem + L.off_b + s * L.b_bytes, inv_scale, p.m, lane, W_FULL(s), [&](int r, float (&v)[4])
+            I8_WAITCNT(wf_a, bars.W_EMPTY(s), ph ^ 1);
+            mbar_wait<64>(bars.W_EMPTY(s), ph ^ 1);
+            i8_write_digit_tile<MR>(smem + L.off_b + s * L.b_bytes, inv_scale, p.m, lane, bars.W_FULL(s), [&](int r, float (&v)[4])
             {
                 if (cached)
                 {
@@ -380,10 +348,10 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             const uint32_t t0 = sm_clock();
 #endif
             // hand the sub-segment's accumulators to the epilogue
-            mbar_wait(D_EMPTY(dbuf), dphase ^ 1);
+            mbar_wait(bars.D_EMPTY(dbuf), dphase ^ 1);
             i8_hand_off<MR>(s_d, s_dt, dbuf, g, nh, wq, lane, acc, t_lo, t_hi);
             __syncwarp();
-            if (lane == 0) mbar_arrive(D_FULL(dbuf));
+            if (lane == 0) mbar_arrive(bars.D_FULL(dbuf));
             dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
 #ifdef EXL3B_TC_DEBUG
             t_ho += sm_clock() - t0;
@@ -397,25 +365,25 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             if (att)
             {
                 // the release wait below, taken apart: mbar_wait_ready<32>
-                if (!mbar_test_wait(W_FULL(s), sph))
+                if (!mbar_test_wait(bars.W_FULL(s), sph))
                 {
                     wait_info = 1u << 31;
                     uint32_t ns = 32, polls = 0;
                     unsigned long long t0 = 0;
-                    while (!mbar_try_wait(W_FULL(s), sph))
+                    while (!mbar_try_wait(bars.W_FULL(s), sph))
                     {
                         __nanosleep(ns); wait_info += ns; if (ns < 512u) ns <<= 1;
-                        poll_watchdog<1023u>(polls, t0, "mbarrier", (int) W_FULL(s), sph);
+                        poll_watchdog<1023u>(polls, t0, "mbarrier", (int) bars.W_FULL(s), sph);
                     }
                 }
             }
             else
 #endif
-            mbar_wait_ready<32>(W_FULL(s), sph);                             // the unit's weights and activation digits
+            mbar_wait_ready<32>(bars.W_FULL(s), sph);                             // the unit's weights and activation digits
 #ifdef EXL3B_TC_DEBUG
             const uint32_t t_out = sm_clock();
 #endif
-            if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) { stamp(3); stamp(4); }
+            if (u == 0 && warp == TC_DEC_WARP0 && lane == 0) { tc_stamp(p.dbg, 3); tc_stamp(p.dbg, 4); }
             const uint32_t* wst = reinterpret_cast<const uint32_t*>(smem + s * L.w_bytes);
 #ifdef EXL3B_TC_DEBUG
             // slots 48 + 4 g + j: SM clock before (low word) and after (high word) the wait of the group's unit j < 4
@@ -438,8 +406,8 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
 #endif
             i8_unit_mma<K, MR>(wst, desc0 + (uint64_t) ((s * L.b_bytes) >> 4), tl, lane, acc, clk, digit_sums);
             __syncwarp();
-            if (lane == 0) mbar_arrive(W_EMPTY(s));
-            if (u == n_units - 1 && wq == 0 && lane == 0) stamp(10);
+            if (lane == 0) mbar_arrive(bars.W_EMPTY(s));
+            if (u == n_units - 1 && wq == 0 && lane == 0) tc_stamp(p.dbg, 10);
 #ifdef EXL3B_TC_DEBUG
             if (att && du >= 1 && du <= 4)
             {
@@ -619,13 +587,13 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             for (int done = 0; done < seg; )
             {
                 const int sub = (seg - done) < I8_SUB_UNITS ? (seg - done) : I8_SUB_UNITS;
-                mbar_wait<32>(D_FULL(dbuf), dphase);
-                if (et == 0 && u + seg >= n_units) stamp(7);
+                mbar_wait<32>(bars.D_FULL(dbuf), dphase);
+                if (et == 0 && u + seg >= n_units) tc_stamp(p.dbg, 7);
                 // the prologue result is needed here too: the first D_FULL orders it (the MMA warps only get operands after the
                 // transform warps passed the prologue barrier)
                 i8_drain<MR>(s_d, s_dt, dbuf, col, p.m, [&](int r) { return i8_over_qmax(__uint_as_float(s_absmax[r])); }, facc);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(D_EMPTY(dbuf));
+                if (lane == 0) mbar_arrive(bars.D_EMPTY(dbuf));
                 dbuf ^= 1; if (dbuf == 0) dphase ^= 1;
                 done += sub;
             }
@@ -640,18 +608,18 @@ __device__ __forceinline__ void gemm_tc_i8_body(const TcParams& p, const CUtenso
             {
                 // contributor: the exchange slots of this matrix's CTA group start at cta0
                 i8_splitk_publish<MR>(parts, cta0 + cta, facc, p.m, col);
-                if (et == 0 && u + seg >= n_units) stamp(11);
+                if (et == 0 && u + seg >= n_units) tc_stamp(p.dbg, 11);
             }
             else
             {
                 // reducer; its slots are re-armed for the launch that uses this exchange buffer next (8 launches from now)
                 i8_splitk_reduce<MR>(parts, cta0, c_a, c_b, facc, p.m, col, tile);
-                if (et == 0 && u + seg >= n_units) stamp(13);
+                if (et == 0 && u + seg >= n_units) tc_stamp(p.dbg, 13);
                 emit_rows(strip);
             }
             u += seg;
         }
-        if (et == 0) stamp(8);
+        if (et == 0) tc_stamp(p.dbg, 8);
     }
 }
 

@@ -1,7 +1,7 @@
 // The unit pipeline of the int8 codebook path (mul1, m <= 8): the data formats and protocols that the single-GEMM body
 // (gemm_tc_i8_body.cuh: plain, row-parallel AR and routed kernels) and the persistent chain kernel (chain_i8.cu) share --
-// the digit tile and its K order, one unit's decode + wgmma, the accumulator hand-off to the epilogue, the mul1 reassembly
-// and the sentinel split-K exchange.  The kernels keep their own barrier waits, which they order differently.
+// the ring's barrier block, the digit tile and its K order, one unit's decode + wgmma, the accumulator hand-off to the
+// epilogue, the mul1 reassembly and the sentinel split-K exchange.
 #pragma once
 #include "tc_common.cuh"
 #include "i8_math.cuh"
@@ -32,12 +32,44 @@ __host__ __device__ constexpr int i8_d_bytes(int MR) { return 2 * 2 * 128 * 2 * 
 
 #ifdef __CUDACC__
 
-// Digit tile of one unit, written by one activation warp into the stage's tile at `dst`: row_values(r, v) gives lane's four
-// transformed values k = 4 lane .. 4 lane + 3 of row r < m.  Each value becomes two digits replicated over the 4 product bytes,
-// stored in the wgmma K order; the per-row digit sums go behind the tile.  Then the tile is made visible to the async proxy and
-// the warp arrives on `x_full` (the chain kernel's X_FULL; in the single-GEMM body the stage's W_FULL, which also takes the weights).
+// Barrier block of the unit ring (S = the launch's ring depth), mbarriers at `bar0`:
+//   W_FULL(s)   word s          the stage's weights (the producer's expect_tx) and its digit tile (the digit warp's arrival):
+//                               a decode warp takes one barrier per unit
+//   W_EMPTY(s)  word S + s      the eight decode warps of the unit's group, after their MMAs have read weights and digits;
+//                               the producer and the digit warp wait for it before they refill the stage
+//   D_FULL(b)   word 3 S + 8 + b   accumulator hand-off buffer b written, by every decode warp
+//   D_EMPTY(b)  word 3 S + 10 + b  buffer b drained, by the four epilogue warps
+// end() is the first word after the block, words(S) its size.
+struct I8Bars
+{
+    static constexpr int W_FULL_ARRIVALS = 2, W_EMPTY_ARRIVALS = TC_DEC_WARPS / I8_DEC_GROUPS;
+    static constexpr int D_FULL_ARRIVALS = TC_DEC_WARPS, D_EMPTY_ARRIVALS = 4;
+    __host__ __device__ static constexpr int words(int S) { return 3 * S + 12; }
+    uint32_t bar0;
+    int S;
+    __device__ __forceinline__ uint32_t W_FULL(int s) const { return bar0 + 8u * s; }
+    __device__ __forceinline__ uint32_t W_EMPTY(int s) const { return bar0 + 8u * (S + s); }
+    __device__ __forceinline__ uint32_t D_FULL(int b) const { return bar0 + 8u * (3 * S + 8 + b); }
+    __device__ __forceinline__ uint32_t D_EMPTY(int b) const { return bar0 + 8u * (3 * S + 10 + b); }
+    __device__ __forceinline__ uint32_t end() const { return bar0 + 8u * words(S); }
+    // by the 32 lanes of one warp, one barrier per lane and round; other() runs on the lanes >= 2 (the caller's own
+    // initialisation), then the warp fences the barriers' initialisation
+    template <typename Other>
+    __device__ __forceinline__ void init(int lane, Other&& other) const
+    {
+        for (int s = lane; s < S; s += 32) { mbar_init(W_FULL(s), W_FULL_ARRIVALS); mbar_init(W_EMPTY(s), W_EMPTY_ARRIVALS); }
+        if (lane < 2) { mbar_init(D_FULL(lane), D_FULL_ARRIVALS); mbar_init(D_EMPTY(lane), D_EMPTY_ARRIVALS); }
+        else other();
+        fence_barrier_init();
+    }
+};
+
+// Digit tile of one unit, written by one activation warp into the stage's tile at `dst` after the stage's W_EMPTY:
+// row_values(r, v) gives lane's four transformed values k = 4 lane .. 4 lane + 3 of row r < m.  Each value becomes two digits
+// replicated over the 4 product bytes, stored in the wgmma K order; the per-row digit sums go behind the tile.  Then the tile is
+// made visible to the async proxy and the warp arrives on the stage's `w_full`.
 template <int MR, typename RowValues>
-__device__ __forceinline__ void i8_write_digit_tile(uint8_t* dst, const float (&inv_scale)[MR], int m, int lane, uint32_t x_full,
+__device__ __forceinline__ void i8_write_digit_tile(uint8_t* dst, const float (&inv_scale)[MR], int m, int lane, uint32_t w_full,
                                                     RowValues&& row_values)
 {
     int qsum[MR];
@@ -84,7 +116,7 @@ __device__ __forceinline__ void i8_write_digit_tile(uint8_t* dst, const float (&
     }
     fence_proxy_async_smem();
     __syncwarp();
-    if (lane == 0) mbar_arrive(x_full);
+    if (lane == 0) mbar_arrive(w_full);
 }
 
 #ifdef EXL3B_TC_DEBUG
@@ -137,7 +169,7 @@ struct I8BatchClock
 
 // One unit (128 k x 128 n weights) of a decode warp: lane (chunk, c) decodes tile column `tl`, both halves, of k-tile 4 r + c
 // (r = 0, 1) from the weight stage `wst` straight into wgmma A fragments, 8 wgmma.m64nNk32 per r against the digit tile at
-// `desc_s`, into acc.  The caller has waited for both the weights and the digits.  `in_flight()` runs while k-half 0's batch
+// `desc_s`, into acc.  The caller has waited for the stage's W_FULL.  `in_flight()` runs while k-half 0's batch
 // is in flight (the caller's per-unit bookkeeping; it must not touch acc).  `clk` takes the batches' issue and retirement
 // times (debug timeline).
 template <int K, int MR, typename InFlight>

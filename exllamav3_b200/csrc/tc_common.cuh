@@ -114,27 +114,25 @@ __device__ __forceinline__ int xt_tile_offset(int r, int lane)
     return (((r >> 3) * 16 + 8 * (lane >> 4) + 2 * (lane & 3)) * 8 + (r & 7)) * 16 + 4 * ((lane >> 2) & 3);
 }
 // the two 4-byte halves land 128 B apart (consecutive K-chunks)
-__device__ __forceinline__ uint2 pack_tile_pair(half2 a, half2 b)
-{
-    uint2 o; o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
-    return o;
-}
 __device__ __forceinline__ void store_tile_pair(uint8_t* p, uint2 o)
 {
     *reinterpret_cast<uint32_t*>(p) = o.x;
     *reinterpret_cast<uint32_t*>(p + 128) = o.y;
 }
-// The input transform of lane's four values k = 4 lane .. 4 lane + 3 of one row (raw fp16, one 128-k block per warp):
-// * suh (`suh` points at lane's four scales) -> 128-point Hadamard in fp32 -> * 1/sqrt(128) -> fp16, as a tile pair
+// The input transform (had128_fp16) of lane's four values of one row, `suh` pointing at lane's four scales, as a tile pair
 __device__ __forceinline__ uint2 xt_transform(uint2 raw, const half* suh, int lane)
 {
-    half2 a = *reinterpret_cast<half2*>(&raw.x), b = *reinterpret_cast<half2*>(&raw.y);
     const uint2 scb = *reinterpret_cast<const uint2*>(suh);
-    a = __hmul2(a, *reinterpret_cast<const half2*>(&scb.x));
-    b = __hmul2(b, *reinterpret_cast<const half2*>(&scb.y));
-    float v0 = __low2float(a), v1 = __high2float(a), v2 = __low2float(b), v3 = __high2float(b);
-    had128_warp(v0, v1, v2, v3, lane);
-    return pack_tile_pair(__floats2half2_rn(v0 * R_SCALE, v1 * R_SCALE), __floats2half2_rn(v2 * R_SCALE, v3 * R_SCALE));
+    return had128_fp16(raw, &scb, lane);
+}
+
+// Bring-up timeline of the tensor-core kernels (EXL3B_TC_DEBUG builds, tools/i8_phase_profile.py): the %globaltimer into slot
+// `slot` of this CTA's row of `dbg` (64 u64 per CTA; null: no stamp).  Compiles to nothing in the other builds.
+__device__ __forceinline__ void tc_stamp([[maybe_unused]] unsigned long long* dbg, [[maybe_unused]] int slot)
+{
+#ifdef EXL3B_TC_DEBUG
+    if (dbg) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory"); dbg[blockIdx.x * 64 + slot] = t; }
+#endif
 }
 #endif
 
