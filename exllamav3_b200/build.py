@@ -17,7 +17,7 @@ _SUFFIX = os.environ.get("EXL3B_LIB_SUFFIX", "")
 OBJ = os.path.join(HERE, "build" + _SUFFIX)
 LIB = os.path.join(HERE, f"libexl3b200{_SUFFIX}.so")
 
-SOURCES = ["api.cu", "kernels_basic.cu", "reconstruct_tc.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_tc_i8.cu", "gemm_tc_i8_ar.cu", "gemm_tc_i8_routed.cu", "chain_i8.cu", "moe_tc.cu", "act.cu", "encode.cu", "hgemm.cu", "hgemm_tc.cu"]
+SOURCES = ["api.cu", "kernels_basic.cu", "reconstruct_tc.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_tc_i8.cu", "gemm_tc_i8_ar.cu", "gemm_tc_i8_routed.cu", "chain_i8.cu", "moe_tc.cu", "act.cu", "norm.cu", "encode.cu", "hgemm.cu", "hgemm_tc.cu"]
 HEADERS = ["common.cuh", "decode.cuh", "epilogue.cuh", "ptx.cuh", "tc_common.cuh", "gemm_tc_i8_body.cuh", "i8_pipeline.cuh", "f16_pipeline.cuh", "i8_math.cuh", "act.cuh", os.path.join("..", "..", "include", "exl3b200.h")]
 
 NVCC_FLAGS = [

@@ -298,6 +298,75 @@ int exl3b_act_mul(void* stream, const void* g, const void* u, void* a, int64_t n
     return launch_act_mul((cudaStream_t) stream, g, u, (half*) a, (long long) numel, in_fp32 != 0, act, act_limit);
 }
 
+// Elements per load unit of the norm kernels: 8 (16-byte vectors) when dim allows it and every tensor is 16-byte aligned, else 4,
+// which needs 4-element alignment (8 bytes for 16-bit types, 16 for fp32); 0 = misaligned
+static int norm_unit(int dim, const void* const* ptrs, const int* dtypes, int n)
+{
+    bool e8 = dim % 8 == 0, e4 = true;
+    for (int i = 0; i < n; ++i)
+    {
+        if (!ptrs[i]) continue;
+        const uintptr_t p = (uintptr_t) ptrs[i];
+        e8 = e8 && p % 16 == 0;
+        e4 = e4 && p % (dtypes[i] == EXL3B_DTYPE_FP32 ? 16 : 8) == 0;
+    }
+    return e8 ? 8 : (e4 ? 4 : 0);
+}
+
+int exl3b_rms_norm(void* stream, const void* x, const void* w, void* y, void* r, int64_t rows, int dim,
+                   int x_dtype, int w_dtype, int y_dtype, int r_dtype, int res_mode,
+                   float eps, float constant_bias, float constant_scale)
+{
+    EXL3B_CHECK(res_mode >= EXL3B_RES_NONE && res_mode <= EXL3B_RES_IN, EXL3B_ERR_ARG, "rms_norm: res_mode must be 0 (none), 1 (post) or 2 (in), got %d", res_mode);
+    EXL3B_CHECK(rows >= 0 && dim >= 0, EXL3B_ERR_SHAPE, "rms_norm: negative size");
+    EXL3B_CHECK(dim % 4 == 0, EXL3B_ERR_SHAPE, "x dimension -1 must be divisible by 4");
+    if (!w) w_dtype = EXL3B_DTYPE_FP16;
+    if (res_mode != EXL3B_RES_IN) r_dtype = x_dtype;
+    // the reference's table: x fp16 / fp32, w fp16 / bf16, y fp16 / fp32 (fp16 in RES_IN), r fp16 / fp32 (RES_IN) or x's type
+    EXL3B_CHECK((x_dtype == EXL3B_DTYPE_FP16 || x_dtype == EXL3B_DTYPE_FP32) && (w_dtype == EXL3B_DTYPE_FP16 || w_dtype == EXL3B_DTYPE_BF16)
+                && (y_dtype == EXL3B_DTYPE_FP16 || (y_dtype == EXL3B_DTYPE_FP32 && res_mode != EXL3B_RES_IN))
+                && (r_dtype == EXL3B_DTYPE_FP16 || r_dtype == EXL3B_DTYPE_FP32), EXL3B_ERR_ARG, "rms_norm: Invalid datatypes for input/output");
+    if (rows == 0 || dim == 0) return 0;
+    EXL3B_CHECK(dim <= NORM_MAX_DIM, EXL3B_ERR_UNSUPPORTED, "rms_norm: dim %d exceeds the %d elements a row may have", dim, NORM_MAX_DIM);
+    EXL3B_CHECK(res_mode != EXL3B_RES_IN || r, EXL3B_ERR_ARG, "rms_norm: res_mode RES_IN requires residual tensor");
+    EXL3B_CHECK(x && y, EXL3B_ERR_ARG, "rms_norm: null tensor");
+    const void* ptrs[4] = {x, w, y, res_mode == EXL3B_RES_IN ? r : nullptr};
+    const int dts[4] = {x_dtype, w_dtype, y_dtype, r_dtype};
+    const int e = norm_unit(dim, ptrs, dts, 4);
+    EXL3B_CHECK(e, EXL3B_ERR_ARG, "rms_norm: x, w, y and r must be aligned to 4 of their elements");
+    NormArgs a{};
+    a.x = x; a.w = w; a.y = y; a.r = res_mode == EXL3B_RES_IN ? r : nullptr; a.rows = rows; a.dim = dim;
+    a.x_dtype = x_dtype; a.w_dtype = w_dtype; a.y_dtype = y_dtype; a.r_dtype = r_dtype; a.res_mode = res_mode;
+    a.eps = eps; a.bias = constant_bias; a.scale = constant_scale; a.e = e;
+    DevCtx* ctx; int rc = get_ctx(&ctx); if (rc) return rc;
+    return launch_rms_norm((cudaStream_t) stream, a);
+}
+
+int exl3b_gated_rms_norm(void* stream, const void* x, const void* w, void* y, const void* g, int64_t rows, int dim,
+                         int x_dtype, int w_dtype, int y_dtype, int g_dtype, int w_groups, int gate_first,
+                         float eps, float constant_bias)
+{
+    EXL3B_CHECK(rows >= 0 && dim >= 0, EXL3B_ERR_SHAPE, "gated_rms_norm: negative size");
+    EXL3B_CHECK(dim % 4 == 0, EXL3B_ERR_SHAPE, "x dimension -1 must be divisible by 4");
+    EXL3B_CHECK(w_groups >= 1, EXL3B_ERR_ARG, "gated_rms_norm: w_groups must be positive, got %d", w_groups);
+    EXL3B_CHECK(x_dtype == EXL3B_DTYPE_BF16 && (w_dtype == EXL3B_DTYPE_FP32 || w_dtype == EXL3B_DTYPE_BF16)
+                && (y_dtype == EXL3B_DTYPE_FP16 || y_dtype == EXL3B_DTYPE_FP32) && (g_dtype == EXL3B_DTYPE_FP32 || g_dtype == EXL3B_DTYPE_BF16),
+                EXL3B_ERR_ARG, "gated_rms_norm: Invalid datatypes for input/output");
+    if (rows == 0 || dim == 0) return 0;
+    EXL3B_CHECK(dim <= NORM_MAX_DIM, EXL3B_ERR_UNSUPPORTED, "gated_rms_norm: dim %d exceeds the %d elements a row may have", dim, NORM_MAX_DIM);
+    EXL3B_CHECK(x && w && y && g, EXL3B_ERR_ARG, "gated_rms_norm: null tensor");
+    const void* ptrs[4] = {x, w, y, g};
+    const int dts[4] = {x_dtype, w_dtype, y_dtype, g_dtype};
+    const int e = norm_unit(dim, ptrs, dts, 4);
+    EXL3B_CHECK(e, EXL3B_ERR_ARG, "gated_rms_norm: x, w, y and g must be aligned to 4 of their elements");
+    NormArgs a{};
+    a.x = x; a.w = w; a.y = y; a.g = g; a.rows = rows; a.dim = dim;
+    a.x_dtype = x_dtype; a.w_dtype = w_dtype; a.y_dtype = y_dtype; a.g_dtype = g_dtype;
+    a.eps = eps; a.bias = constant_bias; a.w_groups = w_groups; a.gate_first = gate_first != 0; a.e = e;
+    DevCtx* ctx; int rc = get_ctx(&ctx); if (rc) return rc;
+    return launch_gated_rms_norm((cudaStream_t) stream, a);
+}
+
 // exl3b_gemm on the rows fp16(act(G) * U): the path exl3b_gemm takes for (m, k, n, K, cb), restricted to the two kernels with a
 // gated input stage (tag 210 at m <= 4, tag 200 at m <= 8); any other choice is refused, never replaced
 int exl3b_gemm_gated(void* stream, const void* G, const void* U, const void* B, void* C, const void* suh, const void* svh,

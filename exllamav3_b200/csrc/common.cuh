@@ -177,6 +177,21 @@ int launch_mgemm_tc_i8_routed(cudaStream_t stream, DevCtx* ctx, const MGemmArgs&
 // standalone gated activation (act.cu): a = fp16(act(g) * u) elementwise
 int launch_act_mul(cudaStream_t stream, const void* g, const void* u, half* a, long long numel, bool in_fp32, int act, float limit);
 
+// RMSNorm operators (norm.cu); the entry points in api.cu check the arguments and pick e
+constexpr int NORM_MAX_DIM = 16384;    // longest row: it is held in registers from its load to its store
+struct NormArgs
+{
+    const void* x; const void* w; void* y; void* r; const void* g;     // w may be NULL (rms_norm); r: RES_IN only; g: gated only
+    long long rows; int dim;
+    int x_dtype, w_dtype, y_dtype, r_dtype, g_dtype;                    // EXL3B_DTYPE_*
+    int res_mode;                                                       // EXL3B_RES_*
+    float eps, bias, scale;
+    int w_groups, gate_first;
+    int e;                                                              // elements per load unit: 8 (16-byte loads of fp16) or 4
+};
+int launch_rms_norm(cudaStream_t stream, const NormArgs& a);
+int launch_gated_rms_norm(cudaStream_t stream, const NormArgs& a);
+
 int launch_hgemm(cudaStream_t stream, const half* a, const half* b, void* c, int m, int k, int n, bool c_fp32,
                  int64_t c_stride);
 

@@ -11,6 +11,7 @@ behaviour (RuntimeError for shape/dtype violations) as the pybind11 bindings the
     exl3_moe, exl3_moe_max_concurrency         bindings.cpp:209-210
     quantize_tiles, pack_trellis               bindings.cpp:116,119 (the converter's trellis encoder)
     silu_mul, gelu_mul, relu2_mul              exllamav3_ext/activation.cu (gated activations)
+    rms_norm, rms_norm_res_in, gated_rms_norm  exllamav3_ext/bindings.cpp:84-86, norm.cu (RMSNorm)
     BC_GatedMLP, BC_MLP                        exllamav3_ext/libtorch/mlp_bc.h, mlp.cpp (MLP decode blocks)
     exl3_gemm_gated                            this library's own: the down projection with the activation in its input stage
 
@@ -101,6 +102,8 @@ _lib.exl3b_moe_max_concurrency.argtypes = [_i]; _lib.exl3b_moe_max_concurrency.r
 _lib.exl3b_moe_plan.argtypes = [_vp, _i, _i, _i, _i, _i, ctypes.POINTER(MoePlan), _vp, _vp]; _lib.exl3b_moe_plan.restype = _i
 _lib.exl3b_act_mul.argtypes = [_vp] * 4 + [_i64, _i, _i, _f]; _lib.exl3b_act_mul.restype = _i
 _lib.exl3b_gemm_gated.argtypes = [_vp] * 7 + [_i] * 8 + [_f, _i]; _lib.exl3b_gemm_gated.restype = _i
+_lib.exl3b_rms_norm.argtypes = [_vp] * 5 + [_i64] + [_i] * 6 + [_f] * 3; _lib.exl3b_rms_norm.restype = _i
+_lib.exl3b_gated_rms_norm.argtypes = [_vp] * 5 + [_i64] + [_i] * 7 + [_f] * 2; _lib.exl3b_gated_rms_norm.restype = _i
 _lib.exl3b_quantize_tiles.argtypes = [_vp] * 4 + [_i64, _i, _i]; _lib.exl3b_quantize_tiles.restype = _i
 _lib.exl3b_pack_trellis.argtypes = [_vp] * 3 + [_i64, _i]; _lib.exl3b_pack_trellis.restype = _i
 
@@ -875,6 +878,87 @@ class BC_MLP:
             y += dn.bias
         if self.yp is not None:
             d.view(1, self.out_size).copy_(self.yp[:, :self.out_size])
+
+
+# ---- RMSNorm (exllamav3_ext/norm.cu) ---------------------------------------------------------------------------------------
+
+RES_NONE, RES_POST, RES_IN = 0, 1, 2
+_NORM_DTYPES = {torch.half: 0, torch.float: 1, torch.bfloat16: 2}
+
+
+def _norm_operands(name: str, x, y, *more):
+    """Device, contiguity and dtype checks of a norm call; returns (rows, dim, dtype code of each of x, y, *more; None -> 0)."""
+    _need_cuda(x, y, *more)
+    ts = [t for t in (x, y) + more if t is not None]
+    if any(t.device != x.device for t in ts):
+        raise RuntimeError(f"{name}: all tensors must be on one device")
+    if not all(t.is_contiguous() for t in ts):
+        raise RuntimeError(f"{name}: all tensors must be contiguous")
+    if any(t.dtype not in _NORM_DTYPES for t in ts):
+        raise RuntimeError(f"{name}: Invalid datatypes for input/output")
+    dim = x.shape[-1] if x.dim() else 1
+    if dim % 4:
+        raise RuntimeError("x dimension -1 must be divisible by 4")
+    if y.shape != x.shape:
+        raise RuntimeError("x and y have incompatible shapes")
+    rows = x.numel() // dim if dim else 0
+    return (rows, dim) + tuple(0 if t is None else _NORM_DTYPES[t.dtype] for t in (x, y) + more)
+
+
+def _rms_norm(x, w, y, r, epsilon: float, constant_bias: float, constant_scale: float, res_mode: int) -> None:
+    rows, dim, tx, ty, tw, tr = _norm_operands("rms_norm", x, y, w, r)
+    if w is not None and (w.dim() == 0 or w.shape[0] != dim or w.numel() != dim):
+        raise RuntimeError("x and w have incompatible shapes")
+    if res_mode == RES_IN:
+        if r is None:
+            raise RuntimeError("rms_norm: res_mode RES_IN requires residual tensor")
+        if r.shape != x.shape:
+            raise RuntimeError("x and r have incompatible shapes")
+    with torch.cuda.device(x.device):
+        _check(_lib.exl3b_rms_norm(_stream(x), _ptr(x), _ptr(w), _ptr(y), _ptr(r), rows, dim, tx, tw, ty, tr, res_mode,
+                                   float(epsilon), float(constant_bias), float(constant_scale)))
+
+
+def rms_norm(x, w, y, epsilon: float, constant_bias: float, constant_scale: float, span_heads: bool, add_residual: bool) -> None:
+    """
+    y = (x * (w + constant_bias)) * rsqrt(mean(x^2) + epsilon) * constant_scale over the last dimension (over the last two with
+    span_heads), or y += that with add_residual.  x fp16 (clamped to +-65504 where read) or fp32, w fp16 / bf16 / None, y fp16 or
+    fp32 of x's shape and may be x; contiguous, last dimension a multiple of 4 and at most 16384.  exllamav3_ext/norm.cu:429-443.
+    Computed in fp32 with one rounding of the result; a row's result is the same in any call that contains it.
+    """
+    if span_heads:
+        x, y = x.flatten(-2), y.flatten(-2)
+    _rms_norm(x, w, y, None, epsilon, constant_bias, constant_scale, RES_POST if add_residual else RES_NONE)
+
+
+def rms_norm_res_in(x, w, y, r, epsilon: float, constant_bias: float, constant_scale: float) -> None:
+    """
+    The residual add folded into the next norm: r = r + x (rounded to r's dtype, written back), then y = rms_norm(r) as
+    rms_norm.  r fp16 or fp32 of x's shape, y fp16.  exllamav3_ext/norm.cu:461-474.
+    """
+    _rms_norm(x, w, y, r, epsilon, constant_bias, constant_scale, RES_IN)
+
+
+def gated_rms_norm(x, w, y, g, epsilon: float, constant_bias: float, w_groups: int = 1, gate_first: bool = False) -> None:
+    """
+    y = rms_norm(x) * (w + constant_bias) * silu(g), or with gate_first y = rms_norm(x * silu(g)) * (w + constant_bias).  x bf16,
+    w fp32 or bf16 holding w_groups rows of dim (row i of x uses w row i % w_groups), g bf16 or fp32 and y fp16 or fp32 of x's
+    shape; contiguous.  exllamav3_ext/norm.cu:582-678.  silu is computed with expf (the reference uses __expf).
+    """
+    rows, dim, tx, ty, tw, tg = _norm_operands("gated_rms_norm", x, y, w, g)
+    w_groups = int(w_groups)
+    if w_groups < 1:
+        raise RuntimeError("gated_rms_norm: w_groups must be positive")
+    if w_groups == 1:
+        if w.dim() == 0 or w.shape[0] != dim or w.numel() != dim:
+            raise RuntimeError("x and w have incompatible shapes")
+    elif w.numel() != w_groups * dim:
+        raise RuntimeError("gated_rms_norm: w must have w_groups * dim elements")
+    if g.shape != x.shape:
+        raise RuntimeError("x and g have incompatible shapes")
+    with torch.cuda.device(x.device):
+        _check(_lib.exl3b_gated_rms_norm(_stream(x), _ptr(x), _ptr(w), _ptr(y), _ptr(g), rows, dim, tx, tw, ty, tg, w_groups,
+                                         int(bool(gate_first)), float(epsilon), float(constant_bias)))
 
 
 # ---- trellis encoder (the converter's two GPU bindings, modules/quant/exl3_lib/quantize.py) ---------------------------------

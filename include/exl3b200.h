@@ -136,6 +136,40 @@ int exl3b_gemm(void* stream,
 int exl3b_act_mul(void* stream, const void* g, const void* u, void* a, int64_t numel, int in_fp32, int act, float act_limit);
 
 /*
+ * ---- RMSNorm ------------------------------------------------------------------------------------------------------------
+ *
+ * exl3b_rms_norm -- replaces ext.rms_norm and ext.rms_norm_res_in (exllamav3_ext/bindings.cpp:84-85, exllamav3_ext/norm.cu).
+ * Over each of `rows` rows of `dim` elements, in fp32:
+ *   rmf = rsqrt(sum(x^2) / dim + eps) * constant_scale,   v = (x * (w + constant_bias)) * rmf   (v = x * rmf when w is NULL)
+ *   res_mode EXL3B_RES_NONE   y = v
+ *            EXL3B_RES_POST   y = y + v, added in fp32 and rounded once
+ *            EXL3B_RES_IN     r = (x + r) rounded to r's dtype and written back; v is then taken of that r instead of x
+ *   x      fp16 (clamped to +-65504 where read) or fp32;  w  (dim) fp16 or bf16, or NULL;  y  fp16 or fp32, may alias x
+ *   r      (rows, dim) fp16 or fp32, EXL3B_RES_IN only (y fp16 there); ignored otherwise
+ *   dtype codes EXL3B_DTYPE_*; w_dtype is ignored when w is NULL, r_dtype unless EXL3B_RES_IN.  All tensors contiguous.
+ *   dim % 4 == 0 and dim <= 16384; the tensors 16-byte aligned, or, when dim % 8 != 0, aligned to 4 of their elements.
+ *   rows = 0 or dim = 0 launches nothing.  Deterministic: a row's result depends on its own values only.  Returns 0.
+ *
+ * exl3b_gated_rms_norm -- replaces ext.gated_rms_norm (bindings.cpp:86):
+ *   s = silu(g),  gate_first = 0:  y = ((x * (w + constant_bias)) * rmf) * s,  rmf = rsqrt(sum(x^2) / dim + eps)
+ *                 gate_first = 1:  the same with x * s in place of x, and no factor s afterwards
+ *   x bf16 (x_dtype must say so);  w (w_groups, dim) fp32 or bf16, row i uses w row i % w_groups;  g (rows, dim) bf16 or fp32;
+ *   y fp16 or fp32.  Sizes and alignment as exl3b_rms_norm, w_groups >= 1.  Returns 0.
+ */
+#define EXL3B_DTYPE_FP16 0
+#define EXL3B_DTYPE_FP32 1
+#define EXL3B_DTYPE_BF16 2
+#define EXL3B_RES_NONE 0
+#define EXL3B_RES_POST 1
+#define EXL3B_RES_IN 2
+int exl3b_rms_norm(void* stream, const void* x, const void* w, void* y, void* r, int64_t rows, int dim,
+                   int x_dtype, int w_dtype, int y_dtype, int r_dtype, int res_mode,
+                   float eps, float constant_bias, float constant_scale);
+int exl3b_gated_rms_norm(void* stream, const void* x, const void* w, void* y, const void* g, int64_t rows, int dim,
+                         int x_dtype, int w_dtype, int y_dtype, int g_dtype, int w_groups, int gate_first,
+                         float eps, float constant_bias);
+
+/*
  * exl3b_gemm_gated -- exl3b_gemm(exl3b_act_mul(G, U), B, ...) with the activation applied where the GEMM reads its input: the
  * down projection of a gated MLP block without the intermediate tensor.  Bit-identical to exl3b_act_mul into a buffer followed by
  * exl3b_gemm on it, with the same path and grid.
