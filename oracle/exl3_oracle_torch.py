@@ -101,3 +101,95 @@ def mul1_weights(trellis: torch.Tensor, K: int, elems: int = CHUNK_ELEMS) -> np.
     for c0, c1 in column_chunks(k, n, elems):
         out[:, c0:c1] = MUL1_W_TABLE[mul1_bytesum(trellis[:, c0 // 16:c1 // 16], K).cpu().numpy()]
     return out
+
+
+# ---- the prefill sibling's models: W_hat of every codebook, had_r_128, reconstruct_had's fp32-sum model -----------------------
+# Restated from exl3_oracle at its rounding points; tests/test_prefill_host.py holds each equal to its numpy original on the CPU
+# device.  torch rounds fp64 -> fp16 through fp32 (two roundings), so every fp16 result below is formed from an fp32 value that
+# is exact or is the numpy model's own fp32 intermediate: an fp16 x fp16 product and a decode's two-half sum fit in 24 bits.
+
+DECODE_TABLES = {cb: orc.decode_values(np.arange(65536, dtype=np.uint16), cb) for cb in range(3)}    # state -> fp16 W_hat
+
+
+def decode_weights(trellis: torch.Tensor, K: int, cb: int, elems: int = CHUNK_ELEMS) -> torch.Tensor:
+    """W_hat (k, n) fp16 on trellis's device, bit for bit exl3_oracle.reconstruct(trellis, K, cb) (any codebook)."""
+    dev = trellis.device
+    k, n = trellis.shape[0] * 16, trellis.shape[1] * 16
+    table = torch.from_numpy(DECODE_TABLES[cb]).to(dev)
+    perm = torch.from_numpy(orc._PERM).to(dev)
+    out = torch.empty((k, n), dtype=torch.half, device=dev)
+    for c0, c1 in column_chunks(k, n, elems):
+        v = table[unpack_states(trellis[:, c0 // 16:c1 // 16], K)]
+        tiles = torch.empty_like(v)
+        tiles[..., perm] = v
+        tk, tn, _ = tiles.shape
+        out[:, c0:c1] = tiles.view(tk, tn, 16, 16).permute(0, 2, 1, 3).reshape(tk * 16, tn * 16)
+        del v, tiles
+    return out
+
+
+def hmul(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """fp16 * fp16 -> fp16 with one rounding (exl3_oracle._hmul): the product is exact in fp32."""
+    return (a.float() * b.float()).half()
+
+
+def fwht128_f32(x: torch.Tensor) -> torch.Tensor:
+    """exl3_oracle.fwht128_f32 on fp32 (..., 128): the same butterflies, width 1, 2, 4 ... 64."""
+    assert x.dtype == torch.float32 and x.shape[-1] == 128
+    lead, v, w = x.shape[:-1], x, 1
+    while w < 128:
+        v = v.reshape(*lead, 128 // (2 * w), 2, w)
+        v = torch.stack((v[..., 0, :] + v[..., 1, :], v[..., 0, :] - v[..., 1, :]), dim=-2)
+        w *= 2
+    return v.reshape(*lead, 128)
+
+
+def had_r_128(x: torch.Tensor, pre_scale=None, post_scale=None, rows: int = 4096) -> torch.Tensor:
+    """exl3_oracle.had_r_128 at scale 1 for fp16 x (pre- or post-scale) and fp32 x (post-scale only), in row chunks."""
+    r_scale = float(orc.R_SCALE_F32)
+    if x.dtype == torch.float32:
+        assert pre_scale is None, "the fp32 pre-scale path (fma contraction) is exl3_oracle.had_r_128's alone"
+    out = torch.empty_like(x)
+    m, c = x.shape
+    for r0 in range(0, m, rows):
+        v = x[r0:r0 + rows]
+        if pre_scale is not None:
+            v = hmul(v, pre_scale[None, :])
+        h = fwht128_f32(v.float().reshape(-1, c // 128, 128)).reshape(-1, c) * r_scale
+        if x.dtype == torch.float16:
+            o = h.half()
+            out[r0:r0 + rows] = hmul(o, post_scale[None, :]) if post_scale is not None and pre_scale is None else o
+        else:
+            out[r0:r0 + rows] = h * post_scale.float()[None, :] if post_scale is not None else h
+    return out
+
+
+def reconstruct_had_model(trellis: torch.Tensor, suh: torch.Tensor, svh: torch.Tensor, K: int, cb: int, n_offset: int = 0,
+                          n: int | None = None, elems: int = CHUNK_ELEMS // 4):
+    """
+    exl3_oracle.reconstruct_had_fp32_model of output columns [n_offset, n_offset + n), on the device in column chunks: returns
+    (w, pre, t_step): the fp16 weights, their value before the suh / svh multiplies, and per row and 128-column block the largest
+    fp16 step of the intermediate tile times fp32(1/sqrt(128)), in fp32 (k, n / 128): what one flipped rounding of that tile
+    moves pre by.  svh is the full vector (indexed by column).
+    Each 128-point sum of fp16 values is exact in fp64 in any order (47 significant bits at most), so the fp64 matmuls give
+    numpy's sums bit for bit.
+    """
+    dev = trellis.device
+    k = trellis.shape[0] * 16
+    n = trellis.shape[1] * 16 - n_offset if n is None else n
+    H = torch.from_numpy(orc.hadamard_matrix_128()).to(dev)
+    r_scale = float(orc.R_SCALE_F32)
+    w_out = torch.empty((k, n), dtype=torch.half, device=dev)
+    pre = torch.empty_like(w_out)
+    t_step = torch.empty((k, n // 128), dtype=torch.float32, device=dev)
+    for c0, c1 in column_chunks(k, n, elems):
+        w = decode_weights(trellis[:, (n_offset + c0) // 16:(n_offset + c1) // 16], K, cb).double()
+        c = c1 - c0
+        t = ((H @ w.view(k // 128, 128, c)).reshape(k, c).float() * r_scale).half()
+        p = ((t.double().view(k, c // 128, 128) @ H).reshape(k, c).float() * r_scale).half()
+        pre[:, c0:c1] = p
+        _, e = torch.frexp(t.float().abs().view(k, c // 128, 128).amax(-1))
+        t_step[:, c0 // 128:c1 // 128] = torch.exp2((e - 11).clamp(min=-24).float()) * r_scale
+        w_out[:, c0:c1] = hmul(hmul(p, suh[:, None]), svh[None, n_offset + c0:n_offset + c1])
+        del w, t, p
+    return w_out, pre, t_step
